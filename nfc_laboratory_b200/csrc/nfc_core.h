@@ -244,15 +244,57 @@ NFC_HD bool gate_open(float adiff, float env)
 // ---------------------------------------------------------------------------------------------------------------------
 // TAPS selects how the search-mode detectors fetch their ring taps (device latency hiding, no semantics):
 //   0  where the reference reads them (one dependent ring access after the other)
-//   2  all taps of the step are loaded up front (independent loads in flight together) and handed to the detectors;
-//      locked lanes other than NFC-A poll frames get prefetch hints for their next step
-struct SearchTaps
+//   2  staged one step ahead (Machine::stage_advance): the taps step k + 1 reads are requested during step k into a
+//      per-lane stage -- shared memory filled by cp.async on the device, a plain copy on the host -- and the taps of
+//      delay 1 are forwarded from the write that produces them; locked lanes other than NFC-A poll frames get prefetch
+//      hints for their next step
+// Word index of a tap inside one stage buffer.  The locked NFC-A poll decoder uses the words of its own rate.
+enum : u32
 {
-   float xa0[3], xa1[3], ca2[3], ca3[3]; // NFC-A: x[t-sdd], x[t-sdd-p2], C[fp2], C[fp3] per rate
-   float wb[2];                          // NFC-B: w[t-sdd] per rate
-   float xf1[2], cf2[2], cf3[2];         // NFC-F 212 / 424: x[t-p2], C[fp2], C[fp3]
-   float xv0, xv1, cv2;                  // NFC-V: x[t-sdd], x[t-sdd-p2], C[fp2]
+   TAP_XA0 = 0,   // NFC-A x[t-sdd] per rate (rate 0 has sdd == 0: the current sample, never staged)
+   TAP_XA1 = 3,   // NFC-A x[t-sdd-p2]
+   TAP_CA2 = 6,   // NFC-A C[fp2]
+   TAP_WB = 9,    // NFC-B w[t-sdd] per rate (rate 0: the current edge value, never staged)
+   TAP_XF1 = 11,  // NFC-F 212 / 424 x[t-p2]
+   TAP_CF2 = 13,  // NFC-F C[fp2]
+   TAP_XV0 = 15,  // NFC-V x[t-sdd]
+   TAP_XV1 = 16,  // NFC-V x[t-sdd-p2]
+   TAP_CV2 = 17,  // NFC-V C[fp2]
+   TAP_FWD = 18,  // forwarded C[fp3] (slot c - 1, written by the previous step): NFC-A rates 0..2, then NFC-F 212 / 424
+   TAP_COUNT = 23
 };
+
+// threads per block of the kernel that stages taps (nfc_decode.cuh lanes_kernel): the word stride of its stage
+#define NFCB200_LANE_THREADS 128
+
+// A tap is requested one step before it is read, before that step writes its own ring slots, so every requested tap
+// must be at least two steps old when it is read.  True when that holds at the periods of P; otherwise nothing is staged.
+NFC_HD bool taps_stageable(const Params &P)
+{
+   bool ok = true;
+   for (int r = 0; r < 3; r++)
+   {
+      const RateParams &b = P.A[r];
+      ok = ok && (b.sdd == 0 || b.sdd >= 2) && b.sdd + b.p2 >= 2 && b.p1 >= b.p2 + 2; // C[fp2] is p1 - p2 steps old
+   }
+   for (int r = 0; r < 2; r++)
+      ok = ok && (P.B[r].sdd == 0 || P.B[r].sdd >= 2);
+   for (int r = 1; r <= 2; r++)
+   {
+      const RateParams &b = P.F[r];
+      ok = ok && b.sdd + b.p2 >= 2 && b.p1 >= b.p2 + 2;
+   }
+   return ok && P.V.sdd >= 2 && P.V.p1 >= P.V.p2 + 2;
+}
+
+#if defined(NFCB200_CHECK_TAPS)
+// development check: every staged tap that is used is compared with a direct ring read (nfcb200.cu reports the counts)
+#if defined(__CUDACC__)
+static __device__ unsigned long long nfcb200_taps_used, nfcb200_taps_differ;
+#else
+static unsigned long long nfcb200_taps_used, nfcb200_taps_differ;
+#endif
+#endif
 
 // CG: ring accesses bypass the L1 cache (ld/st.global.cg).  A ring line is written once and read a few times hundreds
 // of steps later -- no L1 reuse -- while the lanes' local state and sample lines live in the same L1.
@@ -292,9 +334,16 @@ struct Machine
    float *rg; // lane scratch (already offset by the lane index on the device)
    u8 *sb;    // 512-byte stream buffer
    SINK &sink;
-   SearchTaps T;      // TAPS == 2: this step's taps
-   bool tapsValid;    // TAPS == 2: T was loaded for this step
-   bool pollTaps;     // TAPS == 2: slots [0] of T hold the taps of the locked NFC-A poll symbol decoder for this step
+   // TAPS == 2: two stage buffers, this step's (F.k & 1) and the next step's; word (buf, tap) at
+   // stage_base()[(buf * TAP_COUNT + tap) * STG_STRIDE].  The device passes the lane's column of a shared-memory array
+   // ([buf][tap][thread]: no bank conflicts); the host build keeps its own.
+   static constexpr u32 STG_STRIDE = STRIDE == 1 ? 1 : NFCB200_LANE_THREADS;
+   float *stg;
+   float ownStage[TAPS == 2 && STRIDE == 1 ? 2 * TAP_COUNT : 1];
+   // STG_ON | kind of this step's stage (bits 0-2) | kind of the next step's (3-5) | forwarded taps present in this
+   // step's (8-12) | in the next step's (16-20).  Kind: 0 nothing staged, KIND_SEARCH, KIND_POLL + NFC-A rate.
+   u32 stgState;
+   static constexpr u32 STG_ON = 1u << 31, KIND_SEARCH = 1, KIND_POLL = 2;
    float curX, curW;  // sample and edge value of the current step (ring slot of delay 0)
    bool slow;         // a detector left its idle fast path during this step: F.busy must be rebuilt
    // feature-fed front end (nfc_wlane.h): the recurrences of nextSample were evaluated by the front pass, the sample rings
@@ -303,9 +352,19 @@ struct Machine
    float featAvg;
 
    NFC_HD Machine(const Params &p, Lane &l, Front &f, float *r, u8 *s, SINK &k)
-      : P(p), L(l), F(f), rg(r), sb(s), sink(k), tapsValid(false), pollTaps(false), curX(0), curW(0), slow(false), featMode(false),
+      : P(p), L(l), F(f), rg(r), sb(s), sink(k), stg(nullptr), stgState(0), curX(0), curW(0), slow(false), featMode(false),
         featAvg(0)
    {
+      if constexpr (TAPS == 2 && STRIDE == 1)
+         stgState = taps_stageable(P) ? STG_ON : 0;
+   }
+
+   // TAPS == 2 on the device: the lane's stage (column threadIdx.x of a [2][TAP_COUNT][NFCB200_LANE_THREADS] array in
+   // shared memory); `stageable` = taps_stageable(P), evaluated once per launch
+   NFC_HD void attach_stage(float *s, bool stageable)
+   {
+      stg = s;
+      stgState = stageable ? STG_ON : 0;
    }
 
    // running sum of a Mod (index = position of the Mod inside Carry: mA, mB, mF, mV are contiguous)
@@ -321,6 +380,7 @@ struct Machine
          F = L.fe;
       refresh_busy();
       slow = false;
+      stage_reset(); // new ring slot labels (k, kbase), rings wiped by the caller
    }
 
    // write the working copy back (suspended lanes: streaming entry point)
@@ -389,6 +449,8 @@ struct Machine
    {
       for (u32 i = 0; i < len; i++)
          RG(off, i) = 0;
+      if (off != NFCB200_OFF_I) // the integration ring is never staged
+         stage_drop();
    }
 
    NFC_HD void clear_bits()
@@ -601,7 +663,7 @@ struct Machine
             Mod &m = L.c.mA[r];
             FI(m) += SMP(NFCB200_OFF_X, b.sdd);
             FI(m) -= SMP(NFCB200_OFF_X, b.sdd + b.p2);
-            RG(b.corr, F.cA[r]) = FI(m);
+            put_corr(r, b.corr, F.cA[r], FI(m));
          }
       if (P.enabled & EN_F)
          for (int r = 1; r <= 2; r++)
@@ -610,7 +672,7 @@ struct Machine
             Mod &m = L.c.mF[r - 1];
             FI(m) += SMP(NFCB200_OFF_X, b.sdd);
             FI(m) -= SMP(NFCB200_OFF_X, b.sdd + b.p2);
-            RG(b.corr, F.cF[r - 1]) = FI(m);
+            put_corr(3 + r - 1, b.corr, F.cF[r - 1], FI(m));
          }
       if (P.enabled & EN_V)
       {
@@ -712,14 +774,14 @@ struct Machine
          corr_points(fp1, b.p1, b.p2, fp2, fp3);
 
          // :246-250
-         const bool hoisted = TAPS == 2 && tapsValid;
-         FI(m) += hoisted ? (b.sdd ? T.xa0[rate] : curX) : SMP(NFCB200_OFF_X, b.sdd);
-         FI(m) -= hoisted ? T.xa1[rate] : SMP(NFCB200_OFF_X, b.sdd + b.p2);
-         RG(b.corr, fp1) = FI(m);
+         const bool hoisted = staged_for(KIND_SEARCH);
+         FI(m) += (hoisted && b.sdd == 0) ? curX : tap(hoisted, TAP_XA0 + rate, SMP(NFCB200_OFF_X, b.sdd));
+         FI(m) -= tap(hoisted, TAP_XA1 + rate, SMP(NFCB200_OFF_X, b.sdd + b.p2));
+         put_corr(rate, b.corr, fp1, FI(m));
 
          // :253-255
-         const float c2 = hoisted ? T.ca2[rate] : RG(b.corr, fp2);
-         const float c3 = hoisted ? T.ca3[rate] : RG(b.corr, fp3);
+         const float c2 = tap(hoisted, TAP_CA2 + rate, RG(b.corr, fp2));
+         const float c3 = fwd_tap(hoisted, rate, RG(b.corr, fp3));
          float s0 = FI(m) - c2;
          float s1 = c2 - c3;
 
@@ -1173,13 +1235,14 @@ struct Machine
       u32 fp1 = F.cA[F.lockRate], fp2, fp3;
       corr_points(fp1, b.p1, b.p2, fp2, fp3);
 
-      const bool hoisted = TAPS == 2 && pollTaps;
-      FI(m) += hoisted ? (b.sdd ? T.xa0[0] : curX) : (float) SMP(NFCB200_OFF_X, b.sdd);
-      FI(m) -= hoisted ? T.xa1[0] : (float) SMP(NFCB200_OFF_X, b.sdd + b.p2);
-      RG(b.corr, fp1) = FI(m);
+      const u32 rate = F.lockRate;
+      const bool hoisted = staged_for(KIND_POLL + rate);
+      FI(m) += (hoisted && b.sdd == 0) ? curX : tap(hoisted, TAP_XA0 + rate, SMP(NFCB200_OFF_X, b.sdd));
+      FI(m) -= tap(hoisted, TAP_XA1 + rate, SMP(NFCB200_OFF_X, b.sdd + b.p2));
+      put_corr(rate, b.corr, fp1, FI(m));
 
-      const float c2 = hoisted ? T.ca2[0] : (float) RG(b.corr, fp2);
-      const float c3 = hoisted ? T.ca3[0] : (float) RG(b.corr, fp3);
+      const float c2 = tap(hoisted, TAP_CA2 + rate, RG(b.corr, fp2));
+      const float c3 = fwd_tap(hoisted, rate, RG(b.corr, fp3));
       float s0 = FI(m) - c2;
       float s1 = c2 - c3;
 
@@ -1379,7 +1442,7 @@ struct Machine
       FI(m) += v;
       FI(m) -= SMP(NFCB200_OFF_I, b.sdd + b.p2);
 
-      RG(b.corr, fp1) = FI(m);
+      put_corr(F.lockRate, b.corr, fp1, FI(m));
 
       s0 = FI(m) - RG(b.corr, fp2);
       s1 = RG(b.corr, fp2) - RG(b.corr, fp3);
@@ -1920,7 +1983,8 @@ struct Machine
          const RateParams &b = P.B[rate];
          Mod &m = L.c.mB[rate];
 
-         float edge = (TAPS == 2 && tapsValid) ? (b.sdd ? T.wb[rate] : curW) : SMP(NFCB200_OFF_W, b.sdd);
+         const bool hoisted = staged_for(KIND_SEARCH);
+         float edge = (hoisted && b.sdd == 0) ? curW : tap(hoisted, TAP_WB + rate, SMP(NFCB200_OFF_W, b.sdd));
 
          // idle fast path (not in the reference): with no SOF search pending the iteration only acts on a falling edge
          // below -envelope * minimumModulationDeep (:283); the per-sample rewrite of searchValueThreshold (:280) is dead
@@ -2647,7 +2711,7 @@ struct Machine
    {
       u32 fp2, fp3;
       corr_points(fp1, b.p1, b.p2, fp2, fp3);
-      RG(b.corr, fp1) = FI(m);
+      put_corr(3 + (u32) (&b - &P.F[1]), b.corr, fp1, FI(m));
       s0 = FI(m) - RG(b.corr, fp2);
       s1 = RG(b.corr, fp2) - RG(b.corr, fp3);
       sd = fabsf(s0 - s1) / (float) b.p2;
@@ -2664,9 +2728,9 @@ struct Machine
          const RateParams &b = P.F[rate];
          Mod &m = L.c.mF[rate - 1];
 
-         const bool hoisted = TAPS == 2 && tapsValid;
+         const bool hoisted = staged_for(KIND_SEARCH);
          FI(m) += (hoisted && b.sdd == 0) ? curX : SMP(NFCB200_OFF_X, b.sdd);
-         FI(m) -= hoisted ? T.xf1[rate - 1] : SMP(NFCB200_OFF_X, b.sdd + b.p2);
+         FI(m) -= tap(hoisted, TAP_XF1 + rate - 1, SMP(NFCB200_OFF_X, b.sdd + b.p2));
 
          // idle fast path (not in the reference): with no search window pending (the residual pulse counter / threshold
          // only matter at a window end) the iteration only acts when correlatedSD > minimumCorrelationValue (:277); the
@@ -2676,9 +2740,9 @@ struct Machine
             u32 fq2, fq3;
             const u32 fq1 = F.cF[rate - 1];
             corr_points(fq1, b.p1, b.p2, fq2, fq3);
-            RG(b.corr, fq1) = FI(m);
-            const float c2 = hoisted ? T.cf2[rate - 1] : RG(b.corr, fq2);
-            const float c3 = hoisted ? T.cf3[rate - 1] : RG(b.corr, fq3);
+            put_corr(3 + rate - 1, b.corr, fq1, FI(m));
+            const float c2 = tap(hoisted, TAP_CF2 + rate - 1, RG(b.corr, fq2));
+            const float c3 = fwd_tap(hoisted, 3 + rate - 1, RG(b.corr, fq3));
             float q0 = FI(m) - c2;
             float q1 = c2 - c3;
             if (fabsf(q0 - q1) < 0.5f * minimumCorrelationValue * (float) b.p2)
@@ -3050,16 +3114,16 @@ struct Machine
       if (fp2 >= b.p1)
          fp2 -= b.p1;
 
-      const bool hoisted = TAPS == 2 && tapsValid && F.lock == LOCK_NONE;
+      const bool hoisted = staged_for(KIND_SEARCH) && F.lock == LOCK_NONE;
 
-      signalData = hoisted ? T.xv0 : SMP(NFCB200_OFF_X, b.sdd);
+      signalData = tap(hoisted, TAP_XV0, SMP(NFCB200_OFF_X, b.sdd));
 
       FI(m) += signalData;
-      FI(m) -= hoisted ? T.xv1 : SMP(NFCB200_OFF_X, b.sdd + b.p2);
+      FI(m) -= tap(hoisted, TAP_XV1, SMP(NFCB200_OFF_X, b.sdd + b.p2));
 
       RG(b.corr, fp1) = FI(m);
 
-      return ((hoisted ? T.cv2 : RG(b.corr, fp2)) - FI(m)) / (float) b.p2;
+      return (tap(hoisted, TAP_CV2, RG(b.corr, fp2)) - FI(m)) / (float) b.p2;
    }
 
    // NfcV::Impl::detectModulation, NfcV.cpp:236-435
@@ -3378,6 +3442,7 @@ struct Machine
       FI(m) -= SMP(NFCB200_OFF_I, b.sdd + b.p1);
 
       RG(b.corr, fp1) = FI(m);
+      stage_drop(); // a slot of the ring's search-mode period (phase cV0, not cV1)
 
       return RG(b.corr, fp2) - FI(m);
    }
@@ -3570,11 +3635,180 @@ struct Machine
    // ------------------------------------------------------------------------------------------------------------------
    // latency hiding for the ring taps (device; no semantics).  A lone ring access costs an L2 / HBM round trip: the lane
    // scratch of all resident warps (852 kB per warp) is far larger than the caches, and every tap is its own 128-byte
-   // line (32 lanes x 4 bytes).  All taps of search mode are at least one step old when they are read (the smallest
-   // delay is period2 of the 424k detectors; slot c - 1 of a correlation ring was written by the previous step), so they
-   // can be fetched before the front end runs: TAPS == 2 loads them into registers back to back (one round trip for
-   // all instead of one each).
+   // line (32 lanes x 4 bytes), written hundreds of steps before it is read.  A warp step lasts far longer than one round
+   // trip, and every tap of search mode and of the NFC-A poll decoder is at least two steps old when it is read, except
+   // slot c - 1 of a correlation ring, which the previous step wrote.  So TAPS == 2 requests the taps of step k + 1 at
+   // the start of step k (cp.async into the stage in shared memory: no registers held while they are in flight) and
+   // forwards the slot c - 1 values from the writes of step k (put_corr).  The tap set is chosen from the state at step
+   // k; step k + 1 uses its stage only when that choice matches what it runs, and reads the rings directly otherwise.
+   // A stage is dropped by every ring write other than the per-step slot writes (zero_ring, V_listen_corr) and by a
+   // restart of the lane (reload_front), so the values used never depend on the prediction (NFCB200_CHECK_TAPS).
    // ------------------------------------------------------------------------------------------------------------------
+   NFC_HD float *stage_base()
+   {
+      if constexpr (STRIDE == 1)
+         return ownStage;
+      return stg;
+   }
+
+   NFC_HD float &stage_word(u32 buf, u32 tap)
+   {
+      return stage_base()[(buf * TAP_COUNT + tap) * STG_STRIDE];
+   }
+
+   // both stages invalid; the requests still in flight land before anything new is requested
+   NFC_HD void stage_reset()
+   {
+      if constexpr (TAPS == 2)
+      {
+#if defined(__CUDA_ARCH__)
+         asm volatile("cp.async.wait_all;" ::: "memory");
+#endif
+         stgState &= STG_ON;
+      }
+   }
+
+   // the next step's stage invalid (a ring write it may have read ahead of)
+   NFC_HD void stage_drop()
+   {
+      if constexpr (TAPS == 2)
+         stgState &= ~(0x1F0038u);
+   }
+
+   // this step's stage holds the tap set `kind`
+   NFC_HD bool staged_for(u32 kind) const
+   {
+      return TAPS == 2 && (stgState & 7u) == kind;
+   }
+
+   // a tap: from this step's stage when `use`, else from the ring
+   NFC_HD float tap(bool use, u32 t, RingRef direct)
+   {
+      if constexpr (TAPS == 2)
+      {
+         if (use)
+         {
+            const float v = stage_word(F.k & 1, t);
+#if defined(NFCB200_CHECK_TAPS)
+            union
+            {
+               float f;
+               u32 u;
+            } a, e;
+            a.f = v;
+            e.f = direct;
+            const bool same = a.u == e.u;
+#if defined(__CUDA_ARCH__)
+            atomicAdd(&nfcb200_taps_used, 1ull);
+            if (!same)
+               atomicAdd(&nfcb200_taps_differ, 1ull);
+#elif !defined(__CUDACC__)
+            nfcb200_taps_used++;
+            nfcb200_taps_differ += same ? 0 : 1;
+#endif
+#endif
+            return v;
+         }
+      }
+      return direct;
+   }
+
+   // slot c - 1 of correlation ring `fwd` (TAP_FWD order): forwarded by the previous step when it wrote it
+   NFC_HD float fwd_tap(bool use, u32 fwd, RingRef direct)
+   {
+      return tap(use && ((stgState >> (8 + fwd)) & 1u), TAP_FWD + fwd, direct);
+   }
+
+   // the per-step write of correlation ring `fwd` (slot c of this step), also forwarded into the next step's stage
+   NFC_HD void put_corr(u32 fwd, u32 off, u32 slot, float v)
+   {
+      RG(off, slot) = v;
+      if constexpr (TAPS == 2)
+      {
+         stage_word((F.k + 1) & 1, TAP_FWD + fwd) = v;
+         stgState |= 1u << (16 + fwd);
+      }
+   }
+
+   // request ring word (off, index) into word `t` of stage buffer `buf`
+   NFC_HD void stage_fetch(u32 buf, u32 t, u32 off, u32 index)
+   {
+      float *dst = &stage_word(buf, t);
+      const float *src = &rg[(off + index) * STRIDE];
+#if defined(__CUDA_ARCH__)
+      asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((u32) __cvta_generic_to_shared(dst)), "l"(src) : "memory");
+#else
+      *dst = *src;
+#endif
+   }
+
+   // the taps the search-mode detectors read at the next step (ring phases and slot labels one step on)
+   NFC_HD void stage_search(u32 buf)
+   {
+      for (int r = 0; r < 3; r++)
+      {
+         const RateParams &b = P.A[r];
+         const u32 c = wrap(F.cA[r] + 1, b.p1);
+         if (b.sdd)
+            stage_fetch(buf, TAP_XA0 + r, NFCB200_OFF_X, slot_at(b.sdd, 1));
+         stage_fetch(buf, TAP_XA1 + r, NFCB200_OFF_X, slot_at(b.sdd + b.p2, 1));
+         stage_fetch(buf, TAP_CA2 + r, b.corr, wrap(c + b.p2, b.p1));
+      }
+      for (int r = 0; r < 2; r++)
+         if (P.B[r].sdd)
+            stage_fetch(buf, TAP_WB + r, NFCB200_OFF_W, slot_at(P.B[r].sdd, 1));
+      for (int r = 1; r <= 2; r++)
+      {
+         const RateParams &b = P.F[r];
+         const u32 c = wrap(F.cF[r - 1] + 1, b.p1);
+         stage_fetch(buf, TAP_XF1 + r - 1, NFCB200_OFF_X, slot_at(b.sdd + b.p2, 1));
+         stage_fetch(buf, TAP_CF2 + r - 1, b.corr, wrap(c + b.p2, b.p1));
+      }
+      const u32 c = wrap(F.cV1 + 1, P.V.p1);
+      stage_fetch(buf, TAP_XV0, NFCB200_OFF_X, slot_at(P.V.sdd, 1));
+      stage_fetch(buf, TAP_XV1, NFCB200_OFF_X, slot_at(P.V.sdd + P.V.p2, 1));
+      stage_fetch(buf, TAP_CV2, P.V.corr, wrap(c + P.V.p2, P.V.p1));
+   }
+
+   // the taps of A_poll_symbol() (the longest-running locked state of an NFC-A capture) at the next step
+   NFC_HD void stage_poll(u32 buf, u32 r)
+   {
+      const RateParams &b = P.A[r];
+      const u32 c = wrap(F.cA[r] + 1, b.p1);
+      if (b.sdd)
+         stage_fetch(buf, TAP_XA0 + r, NFCB200_OFF_X, slot_at(b.sdd, 1));
+      stage_fetch(buf, TAP_XA1 + r, NFCB200_OFF_X, slot_at(b.sdd + b.p2, 1));
+      stage_fetch(buf, TAP_CA2 + r, b.corr, wrap(c + b.p2, b.p1));
+   }
+
+   // start of a step (after front_advance): request the next step's taps, then wait for this step's
+   NFC_HD void stage_advance()
+   {
+      const u32 s = stgState;
+      u32 kind = 0;
+      if (s & STG_ON)
+      {
+         if (F.lock == LOCK_NONE && !(F.k < F.gate)) // the next step is past the detector gate
+            kind = KIND_SEARCH;
+         else if (F.lock == LOCK_A && L.c.t[TECH_A].fs.frameType == FT_Poll)
+            kind = KIND_POLL + F.lockRate;
+      }
+
+      const u32 next = (F.k + 1) & 1;
+      if (kind == KIND_SEARCH)
+         stage_search(next);
+      else if (kind)
+         stage_poll(next, kind - KIND_POLL);
+      else if (F.lock != LOCK_NONE)
+         prefetch_locked_taps(1);
+
+#if defined(__CUDA_ARCH__)
+      asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 1;" ::: "memory");
+#endif
+      // the next step's stage becomes this step's
+      stgState = (s & STG_ON) | ((s >> 3) & 7u) | (kind << 3) | ((s >> 8) & 0x1F00u);
+   }
+
    NFC_HD void prefetch_slot(u32 off, u32 index)
    {
 #if defined(__CUDA_ARCH__)
@@ -3595,43 +3829,6 @@ struct Machine
    NFC_HD u32 slot_at(u32 delay, u32 ahead) const
    {
       return (F.k + F.kbase + ahead - delay) & (NFCB200_RING - 1);
-   }
-
-   NFC_HD void load_search_taps()
-   {
-      for (int r = 0; r < 3; r++)
-      {
-         const RateParams &b = P.A[r];
-         const u32 c = F.cA[r];
-         T.xa0[r] = b.sdd ? RG(NFCB200_OFF_X, slot_at(b.sdd, 0)) : 0.0f;
-         T.xa1[r] = RG(NFCB200_OFF_X, slot_at(b.sdd + b.p2, 0));
-         T.ca2[r] = RG(b.corr, wrap(c + b.p2, b.p1));
-         T.ca3[r] = RG(b.corr, c ? c - 1 : b.p1 - 1);
-      }
-      for (int r = 0; r < 2; r++)
-         T.wb[r] = P.B[r].sdd ? RG(NFCB200_OFF_W, slot_at(P.B[r].sdd, 0)) : 0.0f;
-      for (int r = 1; r <= 2; r++)
-      {
-         const RateParams &b = P.F[r];
-         const u32 c = F.cF[r - 1];
-         T.xf1[r - 1] = RG(NFCB200_OFF_X, slot_at(b.sdd + b.p2, 0));
-         T.cf2[r - 1] = RG(b.corr, wrap(c + b.p2, b.p1));
-         T.cf3[r - 1] = RG(b.corr, c ? c - 1 : b.p1 - 1);
-      }
-      T.xv0 = RG(NFCB200_OFF_X, slot_at(P.V.sdd, 0));
-      T.xv1 = RG(NFCB200_OFF_X, slot_at(P.V.sdd + P.V.p2, 0));
-      T.cv2 = RG(P.V.corr, wrap(F.cV1 + P.V.p2, P.V.p1));
-   }
-
-   // the four taps of A_poll_symbol() (the longest-running locked state of an NFC-A capture), same idea
-   NFC_HD void load_poll_taps()
-   {
-      const RateParams &b = P.A[F.lockRate];
-      const u32 c = F.cA[F.lockRate];
-      T.xa0[0] = b.sdd ? RG(NFCB200_OFF_X, slot_at(b.sdd, 0)) : 0.0f;
-      T.xa1[0] = RG(NFCB200_OFF_X, slot_at(b.sdd + b.p2, 0));
-      T.ca2[0] = RG(b.corr, wrap(c + b.p2, b.p1));
-      T.ca3[0] = RG(b.corr, c ? c - 1 : b.p1 - 1);
    }
 
    // the symbol decoders of a locked lane read a handful of taps at fixed delays of their own rate
@@ -3683,19 +3880,10 @@ struct Machine
    {
       front_advance();
 
-      if (TAPS == 2)
-      {
-         // search mode with the detectors past their gate: fetch every tap now (the envelope gate below is decided by
-         // this step's sample, an unused fetch is harmless); locked lanes get hints for the next step
-         tapsValid = F.lock == LOCK_NONE && !(F.k - 1 < F.gate);
-         pollTaps = F.lock == LOCK_A && L.c.t[TECH_A].fs.frameType == FT_Poll;
-         if (tapsValid)
-            load_search_taps();
-         else if (pollTaps)
-            load_poll_taps();
-         else if (F.lock != LOCK_NONE)
-            prefetch_locked_taps(1);
-      }
+      // the next step's taps are requested now; the envelope gate below is decided by this step's sample and a lane may
+      // lock or unlock during this step, so some requests go unused, which is harmless
+      if constexpr (TAPS == 2)
+         stage_advance();
 
       if (featMode)
          front_feat();

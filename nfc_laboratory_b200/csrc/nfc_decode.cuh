@@ -452,10 +452,11 @@ struct LaneConfig
    uint32_t *overrun_count;
 };
 
-#define LANE_THREADS 128
+#define LANE_THREADS NFCB200_LANE_THREADS
 
-// all taps of a step are fetched up front (Machine TAPS = 2), four resident blocks per SM.  BAIL: the straggler hand-over is
-// compiled in (a separate instantiation: the extra state costs the plain kernel registers -- 219 -> 250 ms when it was not)
+// the ring taps of a step are staged in shared memory one step ahead (Machine TAPS = 2), four resident blocks per SM.
+// BAIL: the straggler hand-over is compiled in (a separate instantiation: the extra state costs the plain kernel registers
+// -- 219 -> 250 ms when it was not)
 template <bool BAIL>
 __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, const __grid_constant__ Params dP)
 {
@@ -469,6 +470,10 @@ __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, co
    constexpr u32 FRONT_STRIDE = (sizeof(Front) / 4) | 1u;
    __shared__ u32 hot[LANE_THREADS * FRONT_STRIDE];
    Front &F = *reinterpret_cast<Front *>(&hot[threadIdx.x * FRONT_STRIDE]);
+
+   // the tap stages of every lane, [buffer][tap][thread]: each thread reads only the words its own requests wrote
+   __shared__ float stage[2 * TAP_COUNT * LANE_THREADS];
+   const bool stageable = taps_stageable(dP);
 
    for (;;)
    {
@@ -510,6 +515,7 @@ __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, co
          lane_begin(L, dP, R.in, R.first, R.begin - R.first);
 
       Machine<32, DeviceSink, 2, false> M(dP, L, F, rg, sb, sink);
+      M.attach_stage(&stage[threadIdx.x], stageable);
       M.reload_front();
 
       const uint64_t streamBase = have ? (uint64_t) R.stream * c.n_samples : 0;
@@ -582,6 +588,9 @@ __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, co
          atomicAdd(c.work, (unsigned long long) stepped);
       }
    }
+
+   // the last step's requests for a step that never came
+   asm volatile("cp.async.wait_all;" ::: "memory");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

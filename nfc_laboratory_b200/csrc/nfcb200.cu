@@ -479,6 +479,21 @@ int nfcb200_create(const nfcb200_config *cfg, nfcb200_handle **out)
       if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, wlanes_kernel, 32, sizeof(WLaneSmem)) == cudaSuccess && perSm > 0)
          h->wlanesPerSm = perSm;
    }
+   {
+      // the persistent thread-lane grid and its scratch are sized from laneBlocks: never more blocks than fit (registers,
+      // and the shared memory of the Front array plus the tap stages)
+      int plain = 0, bail = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&plain, lanes_kernel<false>, LANE_THREADS, 0) == cudaSuccess &&
+          cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bail, lanes_kernel<true>, LANE_THREADS, 0) == cudaSuccess)
+      {
+         const int fit = std::min(plain, bail);
+         if (fit > 0 && fit < h->laneBlocks)
+         {
+            fprintf(stderr, "nfcb200: only %d thread-lane blocks fit per SM (expected %d)\n", fit, h->laneBlocks);
+            h->laneBlocks = fit;
+         }
+      }
+   }
 
    *out = h;
    return 0;
@@ -490,6 +505,16 @@ void nfcb200_destroy(nfcb200_handle *h)
       return;
    cudaSetDevice(h->device);
    cudaStreamSynchronize(h->stream);
+#if defined(NFCB200_CHECK_TAPS)
+   {
+      // totals of the device so far (make DEFS=-DNFCB200_CHECK_TAPS): staged ring taps used, and those that differed from
+      // the ring word they stand for (must be 0)
+      unsigned long long used = 0, differ = 0;
+      cudaMemcpyFromSymbol(&used, nfcb200_taps_used, sizeof(used));
+      cudaMemcpyFromSymbol(&differ, nfcb200_taps_differ, sizeof(differ));
+      fprintf(stderr, "nfcb200 taps check: %llu staged taps used, %llu differ\n", used, differ);
+   }
+#endif
    DevBuf *bufs[] = {&h->samples, &h->flags, &h->bsum, &h->counts, &h->offsets, &h->lanes, &h->queue, &h->segCounts, &h->segOffsets, &h->segs, &h->feats, &h->scratch, &h->sbuf, &h->pool, &h->ext, &h->meta, &h->carryDev, &h->packed, &h->packedExt, &h->packCtr,
                      &h->counters, &h->sState, &h->sScratch, &h->sSbuf, &h->sSamples, &h->sFlags, &h->sBsum, &h->sCounts};
    for (DevBuf *b: bufs)

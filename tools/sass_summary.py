@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Instruction summary of libnfcb200.so per kernel (cuobjdump -sass, no GPU needed): the mnemonics that prove the Hopper
-paths (TMA bulk copy = UBLKCP, mbarrier = SYNCS.*, warp reductions = REDUX / CREDUX, shuffles = SHFL) and the memory mix
+paths (TMA bulk copy = UBLKCP, mbarrier = SYNCS.*, per-thread async copy = LDGSTS, warp reductions = REDUX / CREDUX, shuffles = SHFL) and the memory mix
 (shared LDS / STS vs generic LD / ST vs local LDL / STL).
 
 usage: python tools/sass_summary.py [path to .so] > sass_summary.md
@@ -26,7 +26,8 @@ for ln in out.splitlines():
         op = m.group(1)
         c = counts[kern]
         c["total"] += 1
-        for key, pat in (("UBLKCP (cp.async.bulk)", r"^UBLKCP"), ("SYNCS (mbarrier)", r"^SYNCS"), ("LDS", r"^LDS"), ("STS", r"^STS"),
+        for key, pat in (("UBLKCP (cp.async.bulk)", r"^UBLKCP"), ("SYNCS (mbarrier)", r"^SYNCS"), ("LDGSTS (cp.async)", r"^LDGSTS"),
+                         ("LDS", r"^LDS"), ("STS", r"^STS"),
                          ("LDG / LD.E (global / generic load)", r"^(LDG|LD\.E|LD$)"), ("STG / ST.E (global / generic store)", r"^(STG|ST\.E|ST$)"),
                          ("LDL", r"^LDL"), ("STL", r"^STL"), ("SHFL", r"^SHFL"), ("REDUX / CREDUX", r"^C?REDUX"), ("MUFU", r"^MUFU"),
                          ("FFMA", r"^FFMA"), ("FADD / FMUL", r"^(FADD|FMUL)"), ("BAR / WARPSYNC", r"^(BAR|WARPSYNC)"), ("ATOM / RED", r"^(ATOM|RED)"),
@@ -37,7 +38,7 @@ print("# SASS instruction summary of `%s` (sm_90a, `cuobjdump -sass`)\n" % so)
 print("Static instruction counts per kernel. `UBLKCP` is the TMA bulk copy (`cp.async.bulk`), `SYNCS.*` its mbarrier; no tensor-core")
 print("instruction appears anywhere: the path has no dense contraction.  `-fmad=false`: FFMA only where the source asks for it")
 print("(`__fmaf_rn` in the screening kernel, the IEEE sqrt / div sequences).\n")
-keys = ["total", "UBLKCP (cp.async.bulk)", "SYNCS (mbarrier)", "LDS", "STS", "LDG / LD.E (global / generic load)", "STG / ST.E (global / generic store)", "LDL", "STL",
+keys = ["total", "UBLKCP (cp.async.bulk)", "SYNCS (mbarrier)", "LDGSTS (cp.async)", "LDS", "STS", "LDG / LD.E (global / generic load)", "STG / ST.E (global / generic store)", "LDL", "STL",
         "SHFL", "REDUX / CREDUX", "MUFU", "FFMA", "FADD / FMUL", "BAR / WARPSYNC", "ATOM / RED", "HMMA / UTC*MMA (tensor)"]
 print("| kernel | " + " | ".join(keys) + " |")
 print("|---|" + "---:|" * len(keys))
