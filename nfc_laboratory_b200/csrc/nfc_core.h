@@ -246,9 +246,10 @@ NFC_HD bool gate_open(float adiff, float env)
 //   0  where the reference reads them (one dependent ring access after the other)
 //   2  staged one step ahead (Machine::stage_advance): the taps step k + 1 reads are requested during step k into a
 //      per-lane stage -- shared memory filled by cp.async on the device, a plain copy on the host -- and the taps of
-//      delay 1 are forwarded from the write that produces them; locked lanes other than NFC-A poll frames get prefetch
-//      hints for their next step
-// Word index of a tap inside one stage buffer.  The locked NFC-A poll decoder uses the words of its own rate.
+//      delay 1 are forwarded from the write that produces them; locked lanes other than NFC-A poll frames and NFC-A
+//      106 kbps (ASK) listen frames get prefetch hints for their next step
+// Word index of a tap inside one stage buffer.  The locked NFC-A poll decoder uses the words of its own rate; the locked
+// NFC-A ASK listen decoder (rate 0, sdd == 0) reuses them for I[t-p2] of the integration ring (TAP_XA1) and C[fp2].
 enum : u32
 {
    TAP_XA0 = 0,   // NFC-A x[t-sdd] per rate (rate 0 has sdd == 0: the current sample, never staged)
@@ -277,6 +278,8 @@ NFC_HD bool taps_stageable(const Params &P)
       const RateParams &b = P.A[r];
       ok = ok && (b.sdd == 0 || b.sdd >= 2) && b.sdd + b.p2 >= 2 && b.p1 >= b.p2 + 2; // C[fp2] is p1 - p2 steps old
    }
+   // the ASK listen decoder (rate 0: sdd == 0) reads w of the current step and writes I[t] each step: I[t-p2] is p2 steps old
+   ok = ok && P.A[0].sdd == 0 && P.A[0].p2 >= 2;
    for (int r = 0; r < 2; r++)
       ok = ok && (P.B[r].sdd == 0 || P.B[r].sdd >= 2);
    for (int r = 1; r <= 2; r++)
@@ -288,11 +291,12 @@ NFC_HD bool taps_stageable(const Params &P)
 }
 
 #if defined(NFCB200_CHECK_TAPS)
-// development check: every staged tap that is used is compared with a direct ring read (nfcb200.cu reports the counts)
+// development check: every staged tap that is used is compared with a direct ring read (nfcb200.cu reports the counts);
+// nfcb200_taps_kind counts the used taps by the kind of the stage they came from (Machine::stgState bits 0-2)
 #if defined(__CUDACC__)
-static __device__ unsigned long long nfcb200_taps_used, nfcb200_taps_differ;
+static __device__ unsigned long long nfcb200_taps_used, nfcb200_taps_differ, nfcb200_taps_kind[8];
 #else
-static unsigned long long nfcb200_taps_used, nfcb200_taps_differ;
+static unsigned long long nfcb200_taps_used, nfcb200_taps_differ, nfcb200_taps_kind[8];
 #endif
 #endif
 
@@ -341,9 +345,10 @@ struct Machine
    float *stg;
    float ownStage[TAPS == 2 && STRIDE == 1 ? 2 * TAP_COUNT : 1];
    // STG_ON | kind of this step's stage (bits 0-2) | kind of the next step's (3-5) | forwarded taps present in this
-   // step's (8-12) | in the next step's (16-20).  Kind: 0 nothing staged, KIND_SEARCH, KIND_POLL + NFC-A rate.
+   // step's (8-12) | in the next step's (16-20).  Kind: 0 nothing staged, KIND_SEARCH, KIND_POLL + NFC-A rate,
+   // KIND_LISTEN_ASK + NFC-A rate (only rate 0, 106 kbps, listens with ASK).
    u32 stgState;
-   static constexpr u32 STG_ON = 1u << 31, KIND_SEARCH = 1, KIND_POLL = 2;
+   static constexpr u32 STG_ON = 1u << 31, KIND_SEARCH = 1, KIND_POLL = 2, KIND_LISTEN_ASK = 5;
    float curX, curW;  // sample and edge value of the current step (ring slot of delay 0)
    bool slow;         // a detector left its idle fast path during this step: F.busy must be rebuilt
    // feature-fed front end (nfc_wlane.h): the recurrences of nextSample were evaluated by the front pass, the sample rings
@@ -449,8 +454,7 @@ struct Machine
    {
       for (u32 i = 0; i < len; i++)
          RG(off, i) = 0;
-      if (off != NFCB200_OFF_I) // the integration ring is never staged
-         stage_drop();
+      stage_drop();
    }
 
    NFC_HD void clear_bits()
@@ -1434,18 +1438,22 @@ struct Machine
       u32 fp1 = F.cA[F.lockRate], fp2, fp3;
       corr_points(fp1, b.p1, b.p2, fp2, fp3);
 
-      float data = SMP(NFCB200_OFF_W, b.sdd);
+      const u32 rate = F.lockRate;
+      const bool hoisted = staged_for(KIND_LISTEN_ASK + rate);
+      float data = hoisted ? curW : (float) SMP(NFCB200_OFF_W, b.sdd); // staged only at rate 0, where sdd == 0
       float v = data * data * 10;
 
       SMP(NFCB200_OFF_I, b.sdd) = v;
 
       FI(m) += v;
-      FI(m) -= SMP(NFCB200_OFF_I, b.sdd + b.p2);
+      FI(m) -= tap(hoisted, TAP_XA1 + rate, SMP(NFCB200_OFF_I, b.sdd + b.p2));
 
-      put_corr(F.lockRate, b.corr, fp1, FI(m));
+      put_corr(rate, b.corr, fp1, FI(m));
 
-      s0 = FI(m) - RG(b.corr, fp2);
-      s1 = RG(b.corr, fp2) - RG(b.corr, fp3);
+      const float c2 = tap(hoisted, TAP_CA2 + rate, RG(b.corr, fp2));
+      const float c3 = fwd_tap(hoisted, rate, RG(b.corr, fp3));
+      s0 = FI(m) - c2;
+      s1 = c2 - c3;
    }
 
    // one sample of decodeListenFrameStartAsk, NfcA.cpp:939-1090
@@ -3636,13 +3644,15 @@ struct Machine
    // latency hiding for the ring taps (device; no semantics).  A lone ring access costs an L2 / HBM round trip: the lane
    // scratch of all resident warps (852 kB per warp) is far larger than the caches, and every tap is its own 128-byte
    // line (32 lanes x 4 bytes), written hundreds of steps before it is read.  A warp step lasts far longer than one round
-   // trip, and every tap of search mode and of the NFC-A poll decoder is at least two steps old when it is read, except
-   // slot c - 1 of a correlation ring, which the previous step wrote.  So TAPS == 2 requests the taps of step k + 1 at
-   // the start of step k (cp.async into the stage in shared memory: no registers held while they are in flight) and
+   // trip, and every tap of search mode and of the NFC-A poll and ASK listen decoders is at least two steps old when it
+   // is read, except slot c - 1 of a correlation ring, which the previous step wrote.  So TAPS == 2 requests the taps of
+   // step k + 1 at the start of step k (cp.async into the stage in shared memory: no registers held while in flight) and
    // forwards the slot c - 1 values from the writes of step k (put_corr).  The tap set is chosen from the state at step
    // k; step k + 1 uses its stage only when that choice matches what it runs, and reads the rings directly otherwise.
-   // A stage is dropped by every ring write other than the per-step slot writes (zero_ring, V_listen_corr) and by a
-   // restart of the lane (reload_front), so the values used never depend on the prediction (NFCB200_CHECK_TAPS).
+   // A stage is dropped by every ring write other than the per-step slot writes (zero_ring -- the wipes of the
+   // correlation and integration rings when a listen phase starts or a decoder resets --, V_listen_corr) and by a restart
+   // of the lane (reload_front), so the values used never depend on the prediction (NFCB200_CHECK_TAPS).  A step that
+   // switches from the poll to the listen decoder wipes the rings, and its stage was chosen for the poll decoder anyway.
    // ------------------------------------------------------------------------------------------------------------------
    NFC_HD float *stage_base()
    {
@@ -3700,10 +3710,12 @@ struct Machine
             const bool same = a.u == e.u;
 #if defined(__CUDA_ARCH__)
             atomicAdd(&nfcb200_taps_used, 1ull);
+            atomicAdd(&nfcb200_taps_kind[stgState & 7u], 1ull);
             if (!same)
                atomicAdd(&nfcb200_taps_differ, 1ull);
 #elif !defined(__CUDACC__)
             nfcb200_taps_used++;
+            nfcb200_taps_kind[stgState & 7u]++;
             nfcb200_taps_differ += same ? 0 : 1;
 #endif
 #endif
@@ -3770,14 +3782,16 @@ struct Machine
       stage_fetch(buf, TAP_CV2, P.V.corr, wrap(c + P.V.p2, P.V.p1));
    }
 
-   // the taps of A_poll_symbol() (the longest-running locked state of an NFC-A capture) at the next step
-   NFC_HD void stage_poll(u32 buf, u32 r)
+   // the taps of a locked NFC-A decoder of rate r at the next step: x[t-sdd] when sdd != 0, ring `off` at delay sdd + p2
+   // and C[fp2].  A_poll_symbol() reads the sample ring (off = X); A_listen_ask_integrate() reads the integration ring
+   // (off = I) and the edge value of the current step (rate 0, sdd == 0).
+   NFC_HD void stage_a(u32 buf, u32 r, u32 off)
    {
       const RateParams &b = P.A[r];
       const u32 c = wrap(F.cA[r] + 1, b.p1);
       if (b.sdd)
          stage_fetch(buf, TAP_XA0 + r, NFCB200_OFF_X, slot_at(b.sdd, 1));
-      stage_fetch(buf, TAP_XA1 + r, NFCB200_OFF_X, slot_at(b.sdd + b.p2, 1));
+      stage_fetch(buf, TAP_XA1 + r, off, slot_at(b.sdd + b.p2, 1));
       stage_fetch(buf, TAP_CA2 + r, b.corr, wrap(c + b.p2, b.p1));
    }
 
@@ -3790,15 +3804,23 @@ struct Machine
       {
          if (F.lock == LOCK_NONE && !(F.k < F.gate)) // the next step is past the detector gate
             kind = KIND_SEARCH;
-         else if (F.lock == LOCK_A && L.c.t[TECH_A].fs.frameType == FT_Poll)
-            kind = KIND_POLL + F.lockRate;
+         else if (F.lock == LOCK_A)
+         {
+            const u32 frameType = L.c.t[TECH_A].fs.frameType;
+            if (frameType == FT_Poll)
+               kind = KIND_POLL + F.lockRate;
+            else if (frameType == FT_Listen && F.lockRate == 0) // A_listen_step: ASK at 106 kbps, BPSK above
+               kind = KIND_LISTEN_ASK + F.lockRate;
+         }
       }
 
       const u32 next = (F.k + 1) & 1;
       if (kind == KIND_SEARCH)
          stage_search(next);
+      else if (kind >= KIND_LISTEN_ASK)
+         stage_a(next, kind - KIND_LISTEN_ASK, NFCB200_OFF_I);
       else if (kind)
-         stage_poll(next, kind - KIND_POLL);
+         stage_a(next, kind - KIND_POLL, NFCB200_OFF_X);
       else if (F.lock != LOCK_NONE)
          prefetch_locked_taps(1);
 

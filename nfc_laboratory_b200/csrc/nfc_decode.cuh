@@ -454,6 +454,42 @@ struct LaneConfig
 
 #define LANE_THREADS NFCB200_LANE_THREADS
 
+#if defined(NFCB200_LANE_PROFILE)
+// development build (make DEFS=-DNFCB200_LANE_PROFILE): where the thread lanes' steps and cycles go.  Per state class,
+// [c] warp steps and [NFCB200_PROF_CLASSES + c] clock64() cycles of those warp steps; nfcb200.cu prints and clears them
+// under NFCB200_TRACE.  The lanes of a warp step through one class at a time (one timed pass per class present), so a
+// class's cycles are its own; a warp step therefore costs more than in the plain build, which interleaves the classes.
+enum
+{
+   PROF_GATED,         // search mode before the detector gate (warm-up)
+   PROF_SEARCH,        // search mode past the gate
+   PROF_A_POLL,        // locked NFC-A, poll frame
+   PROF_A_LISTEN0,     // locked NFC-A 106 kbps listen, before the start of frame (A_listen_start_ask)
+   PROF_A_LISTEN1,     // locked NFC-A 106 kbps listen, symbols (A_listen_symbol_ask)
+   PROF_LOCKED,        // every other locked state
+   PROF_BOOK,          // lane_iterate examines retirement / skip-ahead at this step (and then steps)
+   NFCB200_PROF_CLASSES
+};
+static __device__ unsigned long long nfcb200_lane_prof[2 * NFCB200_PROF_CLASSES];
+
+// the class of the step a running lane takes next
+__device__ __forceinline__ uint32_t lane_prof_class(const Front &F, const Lane &L, uint32_t pos, uint32_t n, bool inactive)
+{
+   if (pos >= n || ((pos & 31) == 0 && inactive))
+      return PROF_BOOK;
+   if (F.lock == LOCK_NONE)
+      return F.k < F.gate ? PROF_GATED : PROF_SEARCH; // step_body gates on k - 1 after front_advance() incremented k
+   if (F.lock != LOCK_A)
+      return PROF_LOCKED;
+   const FrameSt &fs = L.c.t[TECH_A].fs;
+   if (fs.frameType == FT_Poll)
+      return PROF_A_POLL;
+   if (fs.frameType == FT_Listen && F.lockRate == 0)
+      return fs.frameStart ? PROF_A_LISTEN1 : PROF_A_LISTEN0;
+   return PROF_LOCKED;
+}
+#endif
+
 // the ring taps of a step are staged in shared memory one step ahead (Machine TAPS = 2), four resident blocks per SM.
 // BAIL: the straggler hand-over is compiled in (a separate instantiation: the extra state costs the plain kernel registers
 // -- 219 -> 250 ms when it was not)
@@ -474,6 +510,15 @@ __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, co
    // the tap stages of every lane, [buffer][tap][thread]: each thread reads only the words its own requests wrote
    __shared__ float stage[2 * TAP_COUNT * LANE_THREADS];
    const bool stageable = taps_stageable(dP);
+
+#if defined(NFCB200_LANE_PROFILE)
+   // the warp's counters, written by its lane 0 and added to nfcb200_lane_prof when the warp is done
+   __shared__ unsigned long long profAll[LANE_THREADS / 32][2 * NFCB200_PROF_CLASSES];
+   unsigned long long *prof = profAll[threadIdx.x >> 5];
+   if (lane == 0)
+      for (uint32_t i = 0; i < 2 * NFCB200_PROF_CLASSES; i++)
+         prof[i] = 0;
+#endif
 
    for (;;)
    {
@@ -553,7 +598,18 @@ __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, co
       // warp-synchronous stepping: kw is the same in all lanes, so is every ring slot label (k + kbase == kw + 1)
       for (uint32_t kw = 0; __any_sync(0xffffffffu, running); kw++)
       {
+#if defined(NFCB200_LANE_PROFILE)
+         const uint32_t cls = running ? lane_prof_class(F, L, pos, n, pos < n && !active(pos)) : NFCB200_PROF_CLASSES;
+         for (uint32_t pc = 0; pc < NFCB200_PROF_CLASSES; pc++)
+         {
+            const uint32_t in = __ballot_sync(0xffffffffu, cls == pc);
+            if (!in)
+               continue;
+            const long long t0 = clock64();
+            if (cls == pc)
+#else
          if (running)
+#endif
          {
             running = lane_iterate(M, L, dP, pos, end, n, kw, stepped, load, active, zero, succ);
 
@@ -568,6 +624,16 @@ __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, co
                }
             }
          }
+#if defined(NFCB200_LANE_PROFILE)
+            __syncwarp();
+            const long long t1 = clock64();
+            if (lane == 0)
+            {
+               prof[pc]++;
+               prof[NFCB200_PROF_CLASSES + pc] += (unsigned long long) (t1 - t0);
+            }
+         }
+#endif
       }
 
       if (BAIL && bailed)
@@ -588,6 +654,12 @@ __global__ void __launch_bounds__(LANE_THREADS, 4) lanes_kernel(LaneConfig c, co
          atomicAdd(c.work, (unsigned long long) stepped);
       }
    }
+
+#if defined(NFCB200_LANE_PROFILE)
+   if (lane == 0)
+      for (uint32_t i = 0; i < 2 * NFCB200_PROF_CLASSES; i++)
+         atomicAdd(&nfcb200_lane_prof[i], prof[i]);
+#endif
 
    // the last step's requests for a step that never came
    asm volatile("cp.async.wait_all;" ::: "memory");

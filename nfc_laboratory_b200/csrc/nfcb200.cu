@@ -509,10 +509,12 @@ void nfcb200_destroy(nfcb200_handle *h)
    {
       // totals of the device so far (make DEFS=-DNFCB200_CHECK_TAPS): staged ring taps used, and those that differed from
       // the ring word they stand for (must be 0)
-      unsigned long long used = 0, differ = 0;
+      unsigned long long used = 0, differ = 0, kind[8] = {};
       cudaMemcpyFromSymbol(&used, nfcb200_taps_used, sizeof(used));
       cudaMemcpyFromSymbol(&differ, nfcb200_taps_differ, sizeof(differ));
-      fprintf(stderr, "nfcb200 taps check: %llu staged taps used, %llu differ\n", used, differ);
+      cudaMemcpyFromSymbol(kind, nfcb200_taps_kind, sizeof(kind));
+      fprintf(stderr, "nfcb200 taps check: %llu staged taps used (search %llu, A poll %llu, A listen %llu), %llu differ\n", used, kind[1],
+              kind[2] + kind[3] + kind[4], kind[5] + kind[6] + kind[7], differ);
    }
 #endif
    DevBuf *bufs[] = {&h->samples, &h->flags, &h->bsum, &h->counts, &h->offsets, &h->lanes, &h->queue, &h->segCounts, &h->segOffsets, &h->segs, &h->feats, &h->scratch, &h->sbuf, &h->pool, &h->ext, &h->meta, &h->carryDev, &h->packed, &h->packedExt, &h->packCtr,
@@ -1023,6 +1025,26 @@ static int decode_resident(nfcb200_handle *h, const void *dSamples, int sigtype,
          fprintf(stderr, "\n");
          tr.mark("(lane run statistics)");
       }
+#if defined(NFCB200_LANE_PROFILE)
+      {
+         // where the thread lanes' warp steps and cycles went in this call (make DEFS=-DNFCB200_LANE_PROFILE)
+         static const char *names[NFCB200_PROF_CLASSES] = {"gated", "search", "A poll", "A listen start", "A listen symbol", "other locked", "retire / skip"};
+         unsigned long long hp[2 * NFCB200_PROF_CLASSES], zero[2 * NFCB200_PROF_CLASSES] = {};
+         cudaMemcpyFromSymbol(hp, nfcb200_lane_prof, sizeof(hp));
+         cudaMemcpyToSymbol(nfcb200_lane_prof, zero, sizeof(zero));
+         unsigned long long steps = 0, cycles = 0;
+         for (int i = 0; i < NFCB200_PROF_CLASSES; i++)
+         {
+            steps += hp[i];
+            cycles += hp[NFCB200_PROF_CLASSES + i];
+         }
+         fprintf(stderr, "[nfcb200] lane profile: class | warp steps | share | cycles / warp step | share of cycles\n");
+         for (int i = 0; i < NFCB200_PROF_CLASSES; i++)
+            fprintf(stderr, "[nfcb200]   %-16s %14llu %6.2f%% %10.0f %6.2f%%\n", names[i], hp[i], steps ? 100.0 * hp[i] / steps : 0.0,
+                    hp[i] ? (double) hp[NFCB200_PROF_CLASSES + i] / hp[i] : 0.0, cycles ? 100.0 * hp[NFCB200_PROF_CLASSES + i] / cycles : 0.0);
+         fprintf(stderr, "[nfcb200]   %-16s %14llu %7s %10.0f\n", "total", steps, "", steps ? (double) cycles / steps : 0.0);
+      }
+#endif
    }
 
    cudaEventRecord(h->ev[4], st);
