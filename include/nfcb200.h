@@ -203,6 +203,26 @@ int nfcb200_emit_records(nfcb200_handle *h, const void *records, uint64_t n_reco
  */
 int nfcb200_pack_frames(const nfcb200_frame *frames, uint64_t n, uint32_t stream_offset, uint8_t *out, uint64_t cap, uint64_t *n_bytes);
 
+/*
+ * FFT spectrum of IQ captures: lab::FourierProcessTask::process (FourierProcessTask.cpp:223-352, the frequency view of the
+ * reference's GUI, topic "signal.fft") at every hop of every stream.  n_streams captures of n_samples each, laid out
+ * [n_streams][n_samples] in `sigtype` format (NFCB200_SIG_IQ_F32 or NFCB200_SIG_IQ_S16; int16 enters as s / 32768.f).
+ * Frame f of stream s is the reference's frame of a buffer that begins at sample f * hop: decimation d = sample_rate / 625000,
+ * 1024 window positions taken as runs of 4 consecutive samples every 4 d samples (the reference's SSE2 selection), the
+ * sin^2 window, a 1024-point forward FFT, magnitudes sqrt(re^2 + im^2), negative frequencies first.  Frames per stream:
+ * n_samples < 1024 d ? 0 : (n_samples - 1024 d) / hop + 1.
+ *   samples_on_device / out_on_device: `samples` / `out` are device pointers on the handle's device, else host memory
+ *   out: [n_streams][*n_frames][1024] float32; cap counts floats.  If it is too small the call returns NFCB200_ERR_CAPACITY
+ *        with *n_frames set and writes nothing.
+ * A magnitude sigtype or a sample rate below 625 000 S/s returns NFCB200_ERR_UNSUPPORTED.  The call returns when `out` is
+ * complete and changes no decode state of the handle (streaming state, carry, stats, block flags, device frames).
+ */
+int nfcb200_spectrum(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams, uint64_t n_samples,
+                     uint32_t sample_rate, uint64_t hop, float *out, int out_on_device, uint64_t cap, uint64_t *n_frames);
+
+/* frames per stream and decimation of nfcb200_spectrum for a shape; host only, no CUDA call */
+int nfcb200_spectrum_shape(uint64_t n_samples, uint32_t sample_rate, uint64_t hop, uint64_t *n_frames, uint32_t *decimation);
+
 const char *nfcb200_last_error(void);
 
 /* library / build identification, e.g. "nfcb200 0.1 sm_90a" */

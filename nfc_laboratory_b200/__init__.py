@@ -14,7 +14,8 @@ from .binding import (  # noqa: F401
     SIG_MAG_S16,
     library_path,
     load_library,
+    spectrum_shape,
 )
 
 __all__ = ["Frame", "NfcB200Error", "NfcDecoder", "SIG_IQ_F32", "SIG_MAG_F32", "SIG_MAG_S16", "SIG_IQ_S16", "library_path",
-           "load_library"]
+           "load_library", "spectrum_shape"]

@@ -77,8 +77,10 @@ EXPORTS = [
     "nfcb200_config_default", "nfcb200_create", "nfcb200_destroy", "nfcb200_configure", "nfcb200_decode_batch",
     "nfcb200_stream_push", "nfcb200_stream_reset", "nfcb200_get_stats", "nfcb200_get_block_flags", "nfcb200_pack_frames",
     "nfcb200_last_error", "nfcb200_version", "nfcb200_device_frames", "nfcb200_emit_records", "nfcb200_stream_pending", "nfcb200_debug_trace", "nfcb200_carry_size", "nfcb200_set_carry",
-    "nfcb200_carry_before", "nfcb200_default_carry",
+    "nfcb200_carry_before", "nfcb200_default_carry", "nfcb200_spectrum", "nfcb200_spectrum_shape",
 ]
+
+SPECTRUM_BINS = 1024
 
 
 def library_path():
@@ -119,6 +121,9 @@ def load_library():
     lib.nfcb200_device_frames.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
     lib.nfcb200_emit_records.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(CFrame),
                                          C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.nfcb200_spectrum.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint64, C.c_void_p, C.c_int,
+                                     C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.nfcb200_spectrum_shape.argtypes = [C.c_uint64, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
     _lib = lib
     return lib
 
@@ -126,6 +131,16 @@ def load_library():
 def _check(lib, rc):
     if rc != 0:
         raise NfcB200Error(rc, lib.nfcb200_last_error().decode("utf-8", "replace"))
+
+
+def spectrum_shape(n_samples, sample_rate, hop=None):
+    """(frames per stream, decimation) of NfcDecoder.spectrum for streams of n_samples; hop=None is the span, 1024 x decimation"""
+    lib = load_library()
+    nf, dec = C.c_uint64(0), C.c_uint32(0)
+    _check(lib, lib.nfcb200_spectrum_shape(int(n_samples), int(sample_rate), 1, None, C.byref(dec)))
+    hop = SPECTRUM_BINS * dec.value if hop is None else int(hop)
+    _check(lib, lib.nfcb200_spectrum_shape(int(n_samples), int(sample_rate), hop, C.byref(nf), None))
+    return int(nf.value), int(dec.value)
 
 
 _SIG_DTYPE = {SIG_IQ_F32: (np.float32, 2), SIG_MAG_F32: (np.float32, 1), SIG_MAG_S16: (np.int16, 1), SIG_IQ_S16: (np.int16, 2)}
@@ -304,6 +319,43 @@ class NfcDecoder:
             t = t[None]
         n_streams, n_samples = t.shape[0], t.shape[1]
         return self.decode_batch_ptr(t.data_ptr(), t.is_cuda, sigtype, n_streams, n_samples, sample_rate, cap)
+
+    def spectrum(self, samples, sigtype, sample_rate, hop=None):
+        """FFT spectrum of the reference's frequency view (lab::FourierProcessTask) every `hop` samples of every stream
+        (hop=None: one frame per span of 1024 x decimation samples).  samples: IQ as numpy [n_streams, n_samples, 2] (or one
+        stream [n_samples, 2]) -> numpy float32 [n_streams, frames, 1024]; a CUDA tensor of the same shape -> a CUDA tensor
+        on the same device.  Bins run from the most negative frequency up (include/nfcb200.h nfcb200_spectrum)."""
+        dtype, comps = _SIG_DTYPE[sigtype]
+        if isinstance(samples, np.ndarray):
+            a = np.ascontiguousarray(samples, dtype=dtype)
+            a = a[None] if a.ndim == comps else a
+            ptr, on_device = a.ctypes.data, False
+        else:
+            import torch
+            a = samples.contiguous()
+            a = a[None] if a.dim() == comps else a
+            if a.is_cuda and a.device.index != self._cfg.device:
+                raise NfcB200Error(-2, "tensor on %s, decoder on cuda:%d" % (a.device, self._cfg.device))
+            ptr, on_device = a.data_ptr(), a.is_cuda
+        n_streams, n_samples = int(a.shape[0]), int(a.shape[1])
+        if hop is None:
+            hop = SPECTRUM_BINS * spectrum_shape(n_samples, sample_rate)[1]
+        n_frames = spectrum_shape(n_samples, sample_rate, hop)[0]
+        if on_device:
+            out = torch.empty((n_streams, n_frames, SPECTRUM_BINS), dtype=torch.float32, device=a.device)
+            torch.cuda.current_stream(a.device).synchronize()  # the library's stream does not wait for torch's
+            self.spectrum_ptr(ptr, True, sigtype, n_streams, n_samples, sample_rate, hop, out.data_ptr(), True, out.numel())
+        else:
+            out = np.empty((n_streams, n_frames, SPECTRUM_BINS), dtype=np.float32)
+            self.spectrum_ptr(ptr, False, sigtype, n_streams, n_samples, sample_rate, hop, out.ctypes.data, False, out.size)
+        return out
+
+    def spectrum_ptr(self, ptr, on_device, sigtype, n_streams, n_samples, sample_rate, hop, out_ptr, out_on_device, cap):
+        """nfcb200_spectrum on raw addresses (host or device, each side as its flag says); returns the frames per stream"""
+        nf = C.c_uint64(0)
+        _check(self._lib, self._lib.nfcb200_spectrum(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams, n_samples, int(sample_rate),
+                                                     int(hop), C.c_void_p(out_ptr), 1 if out_on_device else 0, int(cap), C.byref(nf)))
+        return int(nf.value)
 
     def nextFrames(self, samples, sample_rate=None, sigtype=SIG_MAG_F32, cap=4096):
         """NfcDecoder::nextFrames(SignalBuffer): streaming decode of one capture.  samples=None (an invalid buffer in the

@@ -25,6 +25,7 @@
 
 #include "../../include/nfcb200.h"
 #include "nfc_decode.cuh"
+#include "nfc_spectrum.cuh"
 
 using namespace nfcb200;
 
@@ -256,6 +257,10 @@ struct nfcb200_handle
    bool sInit = false;
    u32 sEmitted = 0;     // frames already returned
    std::vector<nfcb200_frame> sPending; // decoded but not yet delivered (the caller's buffer was too small)
+
+   // nfcb200_spectrum: its own buffers, so that a spectrum call leaves every decode state above as it was
+   DevBuf specTables, specIn, specOut; // twiddles + window (uploaded once), staged host input, staged host output
+   bool specTablesReady = false;
 };
 
 static int setup_params(nfcb200_handle *h, u32 sampleRate)
@@ -518,7 +523,8 @@ void nfcb200_destroy(nfcb200_handle *h)
    }
 #endif
    DevBuf *bufs[] = {&h->samples, &h->flags, &h->bsum, &h->counts, &h->offsets, &h->lanes, &h->queue, &h->segCounts, &h->segOffsets, &h->segs, &h->feats, &h->scratch, &h->sbuf, &h->pool, &h->ext, &h->meta, &h->carryDev, &h->packed, &h->packedExt, &h->packCtr,
-                     &h->counters, &h->sState, &h->sScratch, &h->sSbuf, &h->sSamples, &h->sFlags, &h->sBsum, &h->sCounts};
+                     &h->counters, &h->sState, &h->sScratch, &h->sSbuf, &h->sSamples, &h->sFlags, &h->sBsum, &h->sCounts,
+                     &h->specTables, &h->specIn, &h->specOut};
    for (DevBuf *b: bufs)
       b->release();
    HostBuf *hbufs[] = {&h->hRecs, &h->hExt};
@@ -1319,6 +1325,129 @@ int nfcb200_decode_batch(nfcb200_handle *h, const void *samples, int samples_on_
    if (nf > cap)
       return fail(NFCB200_ERR_CAPACITY, "%llu frames decoded but room for %llu only", (unsigned long long) nf, (unsigned long long) cap);
 
+   return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// FFT spectrum of IQ (FourierProcessTask::process at every hop, nfc_spectrum.cuh)
+// ---------------------------------------------------------------------------------------------------------------------
+int nfcb200_spectrum_shape(uint64_t n_samples, uint32_t sample_rate, uint64_t hop, uint64_t *n_frames, uint32_t *decimation)
+{
+   if (hop == 0)
+      return fail(NFCB200_ERR_INVALID, "hop of 0 samples");
+   if (sample_rate < (uint32_t) SPEC_BANDWIDTH)
+      return fail(NFCB200_ERR_UNSUPPORTED, "sample rate %u is below the spectrum's 625 kHz bandwidth (decimation 0)", sample_rate);
+   const uint32_t dec = spectrum_decimation(sample_rate);
+   if (n_frames)
+      *n_frames = spectrum_frames(n_samples, dec, hop);
+   if (decimation)
+      *decimation = dec;
+   return 0;
+}
+
+static void launch_spectrum(const nfcb200_handle *h, bool s16, const SpecLaunch &L, cudaStream_t st)
+{
+   const uint64_t grid = std::min<uint64_t>(L.count, (uint64_t) h->smCount * SPEC_BLOCKS_PER_SM);
+   if (s16)
+      spectrum_kernel<true><<<(unsigned) grid, SPEC_THREADS, 0, st>>>(L);
+   else
+      spectrum_kernel<false><<<(unsigned) grid, SPEC_THREADS, 0, st>>>(L);
+}
+
+int nfcb200_spectrum(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams, uint64_t n_samples,
+                     uint32_t sample_rate, uint64_t hop, float *out, int out_on_device, uint64_t cap, uint64_t *n_frames)
+{
+   if (!h)
+      return fail(NFCB200_ERR_INVALID, "null handle");
+   if (n_frames)
+      *n_frames = 0;
+   if (sigtype < SIG_IQ_F32 || sigtype > SIG_IQ_S16)
+      return fail(NFCB200_ERR_INVALID, "unknown signal type %d", sigtype);
+   if (!samples || n_streams == 0 || n_samples == 0)
+      return fail(NFCB200_ERR_INVALID, "empty batch");
+   if (cap && !out)
+      return fail(NFCB200_ERR_INVALID, "null spectrum buffer");
+   if (sigtype != SIG_IQ_F32 && sigtype != SIG_IQ_S16)
+      return fail(NFCB200_ERR_UNSUPPORTED, "the spectrum needs IQ samples (FourierProcessTask.cpp:234 skips other buffers)");
+   uint64_t nf = 0;
+   uint32_t dec = 0;
+   int rc = nfcb200_spectrum_shape(n_samples, sample_rate, hop, &nf, &dec);
+   if (rc)
+      return rc;
+   const uint32_t bs = sig_bytes(sigtype);
+   if (samples_on_device && ((uintptr_t) samples % bs))
+      return fail(NFCB200_ERR_INVALID, "device samples not aligned to %u bytes", bs);
+   if (nf > (~0ull / SPEC_LEN) / n_streams)
+      return fail(NFCB200_ERR_UNSUPPORTED, "%llu frames per stream overflow the output size", (unsigned long long) nf);
+   if (n_frames)
+      *n_frames = nf;
+   const uint64_t total = (uint64_t) n_streams * nf;
+   if (total * SPEC_LEN > cap)
+      return fail(NFCB200_ERR_CAPACITY, "%llu spectrum floats needed but room for %llu only", (unsigned long long) (total * SPEC_LEN),
+                  (unsigned long long) cap);
+   if (total == 0)
+      return 0;
+
+   CUDA_TRY(cudaSetDevice(h->device));
+   cudaStream_t st = h->stream;
+
+   if (!h->specTablesReady)
+   {
+      SpecCx tw[SPEC_LEN];
+      float win[SPEC_LEN];
+      spectrum_tables(tw, win);
+      rc = h->specTables.reserve(sizeof(tw) + sizeof(win));
+      if (rc)
+         return rc;
+      CUDA_TRY(cudaMemcpy(h->specTables.ptr, tw, sizeof(tw), cudaMemcpyHostToDevice));
+      CUDA_TRY(cudaMemcpy(h->specTables.as<unsigned char>() + sizeof(tw), win, sizeof(win), cudaMemcpyHostToDevice));
+      h->specTablesReady = true;
+   }
+
+   SpecLaunch L = {};
+   L.n_samples = n_samples;
+   L.hop = hop;
+   L.n_frames = nf;
+   L.decimation = dec;
+   L.tw = h->specTables.as<SpecCx>();
+   L.win = (const float *) (h->specTables.as<SpecCx>() + SPEC_LEN);
+   const bool s16 = sigtype == SIG_IQ_S16;
+
+   // host input is staged a group of whole streams at a time (about 1 GB); host output a group of frames at a time (256 MB)
+   const uint64_t streamBytes = n_samples * bs;
+   const uint32_t chunkStreams = samples_on_device ? n_streams : (uint32_t) std::max<uint64_t>(1, std::min<uint64_t>(n_streams, (1ull << 30) / streamBytes));
+   const uint64_t chunkFrames = 1ull << 16;
+   if (!samples_on_device && (rc = h->specIn.reserve((uint64_t) chunkStreams * streamBytes)))
+      return rc;
+   if (!out_on_device && (rc = h->specOut.reserve(std::min(total, chunkFrames) * SPEC_LEN * sizeof(float))))
+      return rc;
+
+   for (uint32_t s0 = 0; s0 < n_streams; s0 += chunkStreams)
+   {
+      const uint32_t sc = std::min(chunkStreams, n_streams - s0);
+      if (samples_on_device)
+         L.samples = (const unsigned char *) samples + (uint64_t) s0 * streamBytes;
+      else
+      {
+         CUDA_TRY(cudaMemcpyAsync(h->specIn.ptr, (const unsigned char *) samples + (uint64_t) s0 * streamBytes, (uint64_t) sc * streamBytes,
+                                  cudaMemcpyHostToDevice, st));
+         L.samples = h->specIn.ptr;
+      }
+      L.s0 = s0;
+      const uint64_t g1 = (uint64_t) (s0 + sc) * nf;
+      for (uint64_t g0 = (uint64_t) s0 * nf; g0 < g1;)
+      {
+         L.g0 = g0;
+         L.count = out_on_device ? g1 - g0 : std::min(chunkFrames, g1 - g0);
+         L.out = out_on_device ? out + g0 * SPEC_LEN : h->specOut.as<float>();
+         launch_spectrum(h, s16, L, st);
+         CUDA_TRY(cudaGetLastError());
+         if (!out_on_device)
+            CUDA_TRY(cudaMemcpyAsync(out + g0 * SPEC_LEN, h->specOut.ptr, L.count * SPEC_LEN * sizeof(float), cudaMemcpyDeviceToHost, st));
+         g0 += L.count;
+      }
+   }
+   CUDA_TRY(cudaStreamSynchronize(st));
    return 0;
 }
 
