@@ -38,10 +38,21 @@ typedef enum nfcb200_sigtype
    NFCB200_SIG_IQ_F32 = 1,   /* SIGNAL_TYPE_RADIO_IQ: interleaved float32 I,Q (RadioDeviceTask.cpp:547-655 fused in) */
    NFCB200_SIG_MAG_F32 = 2,  /* SIGNAL_TYPE_RADIO_SAMPLES: float32 magnitude (NfcDecoder::nextFrames input)          */
    NFCB200_SIG_MAG_S16 = 3,  /* mono int16 PCM                                                                       */
-   NFCB200_SIG_IQ_S16 = 4    /* interleaved int16 I,Q                                                                */
+   NFCB200_SIG_IQ_S16 = 4,   /* interleaved int16 I,Q                                                                */
+   NFCB200_SIG_LOGIC_F32 = 5,/* SIGNAL_TYPE_LOGIC_SAMPLES, stride 4: float32 IO, CLK, RST, VCC (IsoDecoder input)   */
+   NFCB200_SIG_LOGIC_S16 = 6 /* the same 4 channels as int16 (4-channel 16-bit WAV), read as s / 32768.f              */
 } nfcb200_sigtype;
 
 enum { NFCB200_TECH_A = 0, NFCB200_TECH_B = 1, NFCB200_TECH_F = 2, NFCB200_TECH_V = 3 };
+
+/* frame tech and frame types of the ISO 7816 decoder (lab-data RawFrame.h:41-61) */
+enum
+{
+   NFCB200_TECH_ISO_ANY = 0x0200, NFCB200_TECH_ISO7816 = 0x0201,
+   NFCB200_FRAME_ISO_VCC_LOW = 0x0200, NFCB200_FRAME_ISO_VCC_HIGH = 0x0201, NFCB200_FRAME_ISO_RST_LOW = 0x0202,
+   NFCB200_FRAME_ISO_RST_HIGH = 0x0203, NFCB200_FRAME_ISO_ATR = 0x0210, NFCB200_FRAME_ISO_REQUEST = 0x0211,
+   NFCB200_FRAME_ISO_RESPONSE = 0x0212, NFCB200_FRAME_ISO_EXCHANGE = 0x0213
+};
 
 /* POD mirror of lab::RawFrame (lab-data RawFrame.cpp:26-39); `stream` is the index of the capture in the batch */
 typedef struct nfcb200_frame
@@ -222,6 +233,20 @@ int nfcb200_spectrum(nfcb200_handle *h, const void *samples, int samples_on_devi
 
 /* frames per stream and decimation of nfcb200_spectrum for a shape; host only, no CUDA call */
 int nfcb200_spectrum_shape(uint64_t n_samples, uint32_t sample_rate, uint64_t hop, uint64_t *n_frames, uint32_t *decimation);
+
+/*
+ * ISO 7816 contact smart-card decode: n_streams 4-channel logic captures (IO, CLK, RST, VCC) of n_samples each, laid out
+ * [n_streams][n_samples][4] in `sigtype` format (NFCB200_SIG_LOGIC_F32 or NFCB200_SIG_LOGIC_S16).  Replaces one
+ * lab::IsoDecoder per stream fed the whole capture by one nextFrames() call, then nextFrames({}) (IsoDecoder.cpp:164-215).
+ * Conventions as nfcb200_decode_batch: samples_on_device, frames ordered by (stream, decode order) with `stream` the batch
+ * index, NFCB200_ERR_CAPACITY after filling cap frames with *n_out the number decoded, date_time from config.stream_time.
+ * VCC / RST changes come as tech 0x0200 frames; ATR, PPS, T=0 TPDUs and T=1 blocks as tech 0x0201.  Payloads over 512
+ * bytes are cut there and flagged Truncated (0x08).  A non-logic sigtype or a sample rate of 0 returns NFCB200_ERR_INVALID,
+ * n_samples >= 2^32 - 1 NFCB200_ERR_UNSUPPORTED (the reference's sample clock is 32-bit).  The call changes no NFC decode
+ * state of the handle (streaming state, carry, stats, block flags, device frames).
+ */
+int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams, uint64_t n_samples,
+                                 uint32_t sample_rate, nfcb200_frame *out, uint64_t cap, uint64_t *n_out);
 
 const char *nfcb200_last_error(void);
 

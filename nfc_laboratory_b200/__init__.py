@@ -10,6 +10,8 @@ from .binding import (  # noqa: F401
     NfcDecoder,
     SIG_IQ_F32,
     SIG_IQ_S16,
+    SIG_LOGIC_F32,
+    SIG_LOGIC_S16,
     SIG_MAG_F32,
     SIG_MAG_S16,
     library_path,
@@ -17,5 +19,6 @@ from .binding import (  # noqa: F401
     spectrum_shape,
 )
 
-__all__ = ["Frame", "NfcB200Error", "NfcDecoder", "SIG_IQ_F32", "SIG_MAG_F32", "SIG_MAG_S16", "SIG_IQ_S16", "library_path",
+__all__ = ["Frame", "NfcB200Error", "NfcDecoder", "SIG_IQ_F32", "SIG_MAG_F32", "SIG_MAG_S16", "SIG_IQ_S16", "SIG_LOGIC_F32", "SIG_LOGIC_S16",
+           "library_path",
            "load_library", "spectrum_shape"]

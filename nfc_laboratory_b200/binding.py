@@ -14,6 +14,8 @@ SIG_IQ_F32 = 1
 SIG_MAG_F32 = 2
 SIG_MAG_S16 = 3
 SIG_IQ_S16 = 4
+SIG_LOGIC_F32 = 5
+SIG_LOGIC_S16 = 6
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -73,6 +75,7 @@ class Frame(tuple):
         return tuple(self[1:])
 
 
+# entry points of include/nfcb200.h whose names are letters and underscores; nfcb200_iso7816_decode_batch is bound below
 EXPORTS = [
     "nfcb200_config_default", "nfcb200_create", "nfcb200_destroy", "nfcb200_configure", "nfcb200_decode_batch",
     "nfcb200_stream_push", "nfcb200_stream_reset", "nfcb200_get_stats", "nfcb200_get_block_flags", "nfcb200_pack_frames",
@@ -123,6 +126,8 @@ def load_library():
                                          C.c_uint64, C.POINTER(C.c_uint64)]
     lib.nfcb200_spectrum.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint64, C.c_void_p, C.c_int,
                                      C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.nfcb200_iso7816_decode_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint32, C.c_uint64, C.c_uint32,
+                                                 C.POINTER(CFrame), C.c_uint64, C.POINTER(C.c_uint64)]
     lib.nfcb200_spectrum_shape.argtypes = [C.c_uint64, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
     _lib = lib
     return lib
@@ -143,7 +148,8 @@ def spectrum_shape(n_samples, sample_rate, hop=None):
     return int(nf.value), int(dec.value)
 
 
-_SIG_DTYPE = {SIG_IQ_F32: (np.float32, 2), SIG_MAG_F32: (np.float32, 1), SIG_MAG_S16: (np.int16, 1), SIG_IQ_S16: (np.int16, 2)}
+_SIG_DTYPE = {SIG_IQ_F32: (np.float32, 2), SIG_MAG_F32: (np.float32, 1), SIG_MAG_S16: (np.int16, 1), SIG_IQ_S16: (np.int16, 2),
+              SIG_LOGIC_F32: (np.float32, 4), SIG_LOGIC_S16: (np.int16, 4)}
 
 
 class NfcDecoder:
@@ -356,6 +362,45 @@ class NfcDecoder:
         _check(self._lib, self._lib.nfcb200_spectrum(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams, n_samples, int(sample_rate),
                                                      int(hop), C.c_void_p(out_ptr), 1 if out_on_device else 0, int(cap), C.byref(nf)))
         return int(nf.value)
+
+    def iso7816_decode(self, samples, sigtype, sample_rate, cap=1 << 16, raw=False):
+        """ISO 7816 contact smart-card frames (lab::IsoDecoder) of 4-channel logic captures IO, CLK, RST, VCC: numpy
+        [n_streams, n_samples, 4] (or one stream [n_samples, 4]), float32 for SIG_LOGIC_F32 or int16 for SIG_LOGIC_S16, or a
+        torch tensor of the same shape (a CUDA tensor is decoded where it lies).  Frames are ordered by (stream, time).
+        raw=True returns (CFrame buffer, count) with every field, time_start / time_end / date_time included."""
+        dtype, comps = _SIG_DTYPE[sigtype]
+        if comps != 4:
+            raise NfcB200Error(-2, "signal type %d is not a 4-channel logic format" % sigtype)
+        keep = None
+        if isinstance(samples, np.ndarray):
+            a = np.ascontiguousarray(samples, dtype=dtype)
+            a = a[None] if a.ndim == 2 else a
+            ptr, on_device, keep = a.ctypes.data, False, a
+        else:
+            import torch
+            a = samples.contiguous()
+            a = a[None] if a.dim() == 2 else a
+            if a.is_cuda and a.device.index != self._cfg.device:
+                raise NfcB200Error(-2, "tensor on %s, decoder on cuda:%d" % (a.device, self._cfg.device))
+            want = torch.float32 if dtype == np.float32 else torch.int16
+            if a.dtype != want:
+                raise NfcB200Error(-2, "signal type %d takes %s samples, got a %s tensor" % (sigtype, want, a.dtype))
+            if a.is_cuda:
+                torch.cuda.current_stream(a.device).synchronize()  # the library's stream does not wait for torch's
+            ptr, on_device, keep = a.data_ptr(), a.is_cuda, a
+        if len(keep.shape) != 3 or keep.shape[2] != 4:
+            raise NfcB200Error(-2, "logic samples must be [n_streams, n_samples, 4], got %s" % (tuple(keep.shape),))
+        n_streams, n_samples = int(keep.shape[0]), int(keep.shape[1])
+        while True:
+            buf = self._buffer(cap)
+            n = C.c_uint64(0)
+            rc = self._lib.nfcb200_iso7816_decode_batch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams, n_samples,
+                                                        int(sample_rate), buf, cap, C.byref(n))
+            if rc == -4 and n.value > cap:
+                cap = int(n.value) + 16
+                continue
+            _check(self._lib, rc)
+            return (buf, n.value) if raw else self._convert(buf, n.value)
 
     def nextFrames(self, samples, sample_rate=None, sigtype=SIG_MAG_F32, cap=4096):
         """NfcDecoder::nextFrames(SignalBuffer): streaming decode of one capture.  samples=None (an invalid buffer in the

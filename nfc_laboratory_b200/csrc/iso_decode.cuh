@@ -1,0 +1,321 @@
+/*
+ * iso_decode.cuh -- ISO 7816 contact smart-card decoding of 4-channel logic captures on the device (iso_core.h).
+ *
+ *   iso_edges_kernel<S16>  the dense pass: one CTA per tile of ISO_TILE samples of one stream.  Every sample is read once
+ *                          (one 16-byte load per float sample, one 8-byte load per int16 sample), its flags are computed
+ *                          against the previous sample, and the tile writes, in sample order, its line events (IO / RST /
+ *                          VCC edges: 12-bit offset | flags << 12) and the 12-bit offsets of its CLK falling edges into
+ *                          per-tile slots.  Events beyond a tile's slots (`line_cap`, `clk_cap`) are counted but not
+ *                          written, and the call runs the pass again with room for one of each at every sample: a
+ *                          two-level clock has at most ISO_TILE / 2 falling edges per tile, but a clock with more levels
+ *                          (noise, a staircase, a ramp) can fall on every sample.
+ *   iso_walk_kernel        one warp per stream runs iso_walk() over the tiles' events in order (the lanes evaluate 32
+ *                          clock measurements at a time) and appends its frames to a pool with the stream index and the
+ *                          frame's rank in its stream, and the stream's frame count.
+ *   iso_gather_kernel      moves every pooled frame to its place in (stream, rank) order: the host's scan of the
+ *                          streams' counts gives each stream's first place.
+ */
+#ifndef NFCB200_ISO_DECODE_CUH
+#define NFCB200_ISO_DECODE_CUH
+
+#include <stdint.h>
+
+#include "../../include/nfcb200.h"
+#include "iso_core.h"
+
+namespace nfcb200 {
+
+constexpr uint32_t ISO_TILE = 4096;             // samples per tile (12-bit offsets)
+constexpr uint32_t ISO_THREADS = 256;
+constexpr uint32_t ISO_PER_THREAD = ISO_TILE / ISO_THREADS;
+constexpr uint32_t ISO_CLK_CAP = ISO_TILE / 2;  // CLK falling edges per tile on the first try (a two-level clock fits)
+constexpr uint32_t ISO_LINE_CAP = 256;          // line events per tile on the first try
+
+struct IsoEdgesArgs
+{
+   const void *samples;  // [n_streams][n_samples][4]
+   uint64_t n_samples;
+   uint32_t n_tiles;     // tiles per stream
+   uint32_t line_cap, clk_cap;
+   uint32_t *line;       // [stream][tile][line_cap]
+   uint32_t *line_count; // [stream][tile]
+   uint16_t *clk;        // [stream][tile][clk_cap]
+   uint32_t *clk_count;  // [stream][tile]
+   uint32_t *overflow;   // set when a tile has more line events than line_cap or more CLK falling edges than clk_cap
+};
+
+template <bool S16>
+__device__ __forceinline__ void iso_load(const void *base, uint64_t i, float d[4])
+{
+   if (S16)
+   {
+      const uint2 v = __ldg((const uint2 *) base + i);
+      d[0] = (int16_t) (v.x & 0xFFFF) / 32768.f;
+      d[1] = (int16_t) (v.x >> 16) / 32768.f;
+      d[2] = (int16_t) (v.y & 0xFFFF) / 32768.f;
+      d[3] = (int16_t) (v.y >> 16) / 32768.f;
+   }
+   else
+   {
+      const float4 v = __ldg((const float4 *) base + i);
+      d[0] = v.x;
+      d[1] = v.y;
+      d[2] = v.z;
+      d[3] = v.w;
+   }
+}
+
+template <bool S16>
+__global__ void __launch_bounds__(ISO_THREADS) iso_edges_kernel(const IsoEdgesArgs a)
+{
+   using namespace iso7816;
+   __shared__ uint32_t warpLine[ISO_PER_THREAD][ISO_THREADS / 32], warpClk[ISO_PER_THREAD][ISO_THREADS / 32];
+
+   const uint32_t tile = blockIdx.x, stream = blockIdx.y;
+   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+   const uint64_t t0 = (uint64_t) tile * ISO_TILE;
+   const void *base = S16 ? (const void *) ((const uint2 *) a.samples + (uint64_t) stream * a.n_samples)
+                          : (const void *) ((const float4 *) a.samples + (uint64_t) stream * a.n_samples);
+
+   uint32_t fl[ISO_PER_THREAD];
+#pragma unroll
+   for (uint32_t j = 0; j < ISO_PER_THREAD; j++)
+   {
+      const uint64_t i = t0 + j * ISO_THREADS + threadIdx.x;
+      float d[4] = {0, 0, 0, 0}, l[4] = {0, 0, 0, 0};
+      if (i < a.n_samples)
+      {
+         iso_load<S16>(base, i, d);
+         if (i > 0)
+            iso_load<S16>(base, i - 1, l);
+      }
+      fl[j] = i < a.n_samples ? sample_flags(d, l) : 0u;
+      const uint32_t bl = __ballot_sync(~0u, (fl[j] & F_LINE) != 0), bc = __ballot_sync(~0u, (fl[j] & F_CLK_FALL) != 0);
+      if (lane == 0)
+      {
+         warpLine[j][warp] = __popc(bl);
+         warpClk[j][warp] = __popc(bc);
+      }
+   }
+   __syncthreads();
+   // exclusive scan of the per-(j, warp) counts in sample order, by warp 0
+   __shared__ uint32_t offLine[ISO_PER_THREAD][ISO_THREADS / 32], offClk[ISO_PER_THREAD][ISO_THREADS / 32], total[2];
+   if (warp == 0)
+   {
+      constexpr uint32_t N = ISO_PER_THREAD * (ISO_THREADS / 32), PER = N / 32;
+      uint32_t *wl = &warpLine[0][0], *wc = &warpClk[0][0];
+      uint32_t sl = 0, sc = 0;
+      for (uint32_t k = 0; k < PER; k++)
+      {
+         sl += wl[lane * PER + k];
+         sc += wc[lane * PER + k];
+      }
+      uint32_t il = sl, ic = sc;
+      for (uint32_t o = 1; o < 32; o <<= 1)
+      {
+         const uint32_t vl = __shfl_up_sync(~0u, il, o), vc = __shfl_up_sync(~0u, ic, o);
+         if (lane >= o)
+         {
+            il += vl;
+            ic += vc;
+         }
+      }
+      uint32_t el = il - sl, ec = ic - sc;
+      for (uint32_t k = 0; k < PER; k++)
+      {
+         const uint32_t cl = wl[lane * PER + k], cc = wc[lane * PER + k];
+         (&offLine[0][0])[lane * PER + k] = el;
+         (&offClk[0][0])[lane * PER + k] = ec;
+         el += cl;
+         ec += cc;
+      }
+      if (lane == 31)
+      {
+         total[0] = il;
+         total[1] = ic;
+      }
+   }
+   __syncthreads();
+
+   const uint64_t slot = (uint64_t) stream * a.n_tiles + tile;
+   uint32_t *line = a.line + slot * a.line_cap;
+   uint16_t *clk = a.clk + slot * a.clk_cap;
+   const uint32_t below = (1u << lane) - 1;
+#pragma unroll
+   for (uint32_t j = 0; j < ISO_PER_THREAD; j++)
+   {
+      const uint32_t off = j * ISO_THREADS + threadIdx.x;
+      const bool isLine = (fl[j] & F_LINE) != 0, isClk = (fl[j] & F_CLK_FALL) != 0;
+      const uint32_t bl = __ballot_sync(~0u, isLine), bc = __ballot_sync(~0u, isClk);
+      if (isLine)
+      {
+         const uint32_t k = offLine[j][warp] + __popc(bl & below);
+         if (k < a.line_cap)
+            line[k] = off | (fl[j] & ~F_CLK_FALL) << 12;
+      }
+      if (isClk)
+      {
+         const uint32_t k = offClk[j][warp] + __popc(bc & below);
+         if (k < a.clk_cap)
+            clk[k] = (uint16_t) off;
+      }
+   }
+   if (threadIdx.x == 0)
+   {
+      a.line_count[slot] = total[0];
+      a.clk_count[slot] = total[1];
+      if (total[0] > a.line_cap || total[1] > a.clk_cap)
+         atomicOr(a.overflow, 1u);
+   }
+}
+
+// the event source of iso_walk(): the per-tile slots of one stream, read in tile order
+struct IsoDevEvents
+{
+   const uint32_t *line, *lineCount;
+   const uint16_t *clk;
+   const uint32_t *clkCount;
+   uint32_t nTiles, lineCap, clkCap;
+   uint32_t lt = 0, li = 0, ct = 0, ci = 0;
+
+   __device__ uint32_t line_peek()
+   {
+      while (lt < nTiles && li >= lineCount[lt])
+      {
+         lt++;
+         li = 0;
+      }
+      return lt < nTiles ? lt * ISO_TILE + (line[(uint64_t) lt * lineCap + li] & (ISO_TILE - 1)) : iso7816::NONE;
+   }
+
+   __device__ uint32_t line_pop()
+   {
+      return line[(uint64_t) lt * lineCap + li++] >> 12;
+   }
+
+   __device__ uint32_t clk_nth(uint32_t k)
+   {
+      uint32_t t = ct, i = ci;
+      while (t < nTiles)
+      {
+         const uint32_t n = clkCount[t];
+         if (i < n)
+         {
+            if (k < n - i)
+               return t * ISO_TILE + clk[(uint64_t) t * clkCap + i + k];
+            k -= n - i;
+         }
+         t++;
+         i = 0;
+      }
+      return iso7816::NONE;
+   }
+
+   __device__ void clk_pop()
+   {
+      clk_skip(1);
+   }
+
+   __device__ void clk_skip(uint32_t k)
+   {
+      while (ct < nTiles)
+      {
+         const uint32_t n = clkCount[ct];
+         if (ci + k <= n)
+         {
+            ci += k;
+            return;
+         }
+         k -= n > ci ? n - ci : 0;
+         ct++;
+         ci = 0;
+      }
+   }
+};
+
+struct IsoWalkArgs
+{
+   uint32_t n_streams, stream0, n_samples, n_tiles, line_cap, clk_cap, sample_rate, stream_time;
+   const uint32_t *line, *line_count, *clk_count;
+   const uint16_t *clk;
+   nfcb200_frame *pool;
+   uint32_t pool_cap;
+   uint32_t *pool_count;
+   uint32_t *stream_count; // [n_streams] frames of each stream
+};
+
+struct IsoDevSink
+{
+   const IsoWalkArgs *a;
+   uint32_t stream, rank;
+
+   // every lane of the warp calls this with the same frame; lane 0 writes it
+   __device__ void frame(const iso7816::IsoFrameOut &f)
+   {
+      const uint32_t k = (threadIdx.x & 31) == 0 ? atomicAdd(a->pool_count, 1u) : ~0u;
+      if (k < a->pool_cap)
+      {
+         nfcb200_frame &o = a->pool[k];
+         o.stream = stream;
+         o.tech_type = f.techType;
+         o.frame_type = f.frameType;
+         o.frame_flags = f.frameFlags;
+         o.frame_phase = f.framePhase;
+         o.frame_rate = f.frameRate;
+         o.length = f.length;
+         o.reserved = rank;
+         o.sample_start = f.sampleStart;
+         o.sample_end = f.sampleEnd;
+         o.sample_rate = a->sample_rate;
+         o.time_start = f.timeStart;
+         o.time_end = f.timeEnd;
+         o.date_time = f.dateTime;
+         const uint32_t n = f.length < iso7816::FRAME_BYTES ? f.length : iso7816::FRAME_BYTES;
+         for (uint32_t i = 0; i < ((n + 63) & ~63u); i++)
+            o.data[i] = i < n ? f.data[i] : 0;
+      }
+      rank++;
+   }
+};
+
+// one warp per stream: every lane keeps the same state (iso_walk evaluates clock measurements across the lanes)
+__global__ void __launch_bounds__(32) iso_walk_kernel(const IsoWalkArgs a)
+{
+   const uint32_t s = blockIdx.x;
+   IsoDevEvents ev;
+   ev.line = a.line + (uint64_t) s * a.n_tiles * a.line_cap;
+   ev.lineCount = a.line_count + (uint64_t) s * a.n_tiles;
+   ev.clk = a.clk + (uint64_t) s * a.n_tiles * a.clk_cap;
+   ev.clkCount = a.clk_count + (uint64_t) s * a.n_tiles;
+   ev.nTiles = a.n_tiles;
+   ev.lineCap = a.line_cap;
+   ev.clkCap = a.clk_cap;
+   IsoDevSink sink {&a, a.stream0 + s, 0};
+   iso7816::IsoMachine m;
+   iso7816::iso_init(m, a.sample_rate, a.stream_time);
+   iso7816::iso_walk(m, ev, a.n_samples, sink);
+   if (threadIdx.x == 0)
+      a.stream_count[s] = sink.rank;
+}
+
+// pooled frame k -> out[first[stream - stream0] + rank], the rank field cleared; first[] counts from the chunk's first frame
+__global__ void iso_gather_kernel(const nfcb200_frame *pool, uint32_t count, const uint64_t *first, uint32_t stream0, nfcb200_frame *out)
+{
+   constexpr uint32_t WORDS = sizeof(nfcb200_frame) / 16;
+   static_assert(sizeof(nfcb200_frame) % 16 == 0, "frames move as 16-byte words");
+   const uint32_t lane = threadIdx.x & 31;
+   for (uint64_t k = (blockIdx.x * (uint64_t) blockDim.x + threadIdx.x) / 32; k < count; k += (uint64_t) gridDim.x * blockDim.x / 32)
+   {
+      const nfcb200_frame &f = pool[k];
+      nfcb200_frame *o = out + first[f.stream - stream0] + f.reserved;
+      for (uint32_t w = lane; w < WORDS; w += 32)
+         ((uint4 *) o)[w] = ((const uint4 *) &f)[w];
+      __syncwarp();
+      if (lane == 0)
+         o->reserved = 0;
+   }
+}
+
+} // namespace nfcb200
+
+#endif

@@ -440,10 +440,11 @@ __global__ void __launch_bounds__(SCR_THREADS, 2) screen_kernel(ScreenConfig c, 
       }
       else
       {
-         // plain coalesced 16-byte loads (debug knob; same staging layout)
+         // plain coalesced 16-byte loads (debug knob; same staging layout).  This path also serves batches whose stream
+         // pitch is not a multiple of 16 bytes, where a stream after the first starts unaligned: bytes one at a time
          const unsigned char *src = (const unsigned char *) c.samples + ((uint64_t) g.stream * c.n_samples + (uint64_t) g.lo) * bs;
          unsigned char *dst = s.raw[stage] + (uint32_t) (g.lo - g.base) * bs;
-         uint32_t vec = bytes >> 4;
+         uint32_t vec = (((uintptr_t) src | (uintptr_t) dst) & 15) ? 0 : bytes >> 4;
          for (uint32_t i = tid; i < vec; i += SCR_THREADS)
             ((uint4 *) dst)[i] = __ldg(((const uint4 *) src) + i);
          for (uint32_t i = (vec << 4) + tid; i < bytes; i += SCR_THREADS)

@@ -26,6 +26,7 @@
 #include "../../include/nfcb200.h"
 #include "nfc_decode.cuh"
 #include "nfc_spectrum.cuh"
+#include "iso_decode.cuh"
 
 using namespace nfcb200;
 
@@ -261,6 +262,9 @@ struct nfcb200_handle
    // nfcb200_spectrum: its own buffers, so that a spectrum call leaves every decode state above as it was
    DevBuf specTables, specIn, specOut; // twiddles + window (uploaded once), staged host input, staged host output
    bool specTablesReady = false;
+
+   // nfcb200_iso7816_decode_batch: its own buffers too
+   DevBuf isoIn, isoLine, isoLineCount, isoClk, isoClkCount, isoPool, isoCtr, isoStreamCount, isoFirst, isoOrdered;
 };
 
 static int setup_params(nfcb200_handle *h, u32 sampleRate)
@@ -524,7 +528,8 @@ void nfcb200_destroy(nfcb200_handle *h)
 #endif
    DevBuf *bufs[] = {&h->samples, &h->flags, &h->bsum, &h->counts, &h->offsets, &h->lanes, &h->queue, &h->segCounts, &h->segOffsets, &h->segs, &h->feats, &h->scratch, &h->sbuf, &h->pool, &h->ext, &h->meta, &h->carryDev, &h->packed, &h->packedExt, &h->packCtr,
                      &h->counters, &h->sState, &h->sScratch, &h->sSbuf, &h->sSamples, &h->sFlags, &h->sBsum, &h->sCounts,
-                     &h->specTables, &h->specIn, &h->specOut};
+                     &h->specTables, &h->specIn, &h->specOut, &h->isoIn, &h->isoLine, &h->isoLineCount, &h->isoClk, &h->isoClkCount,
+                     &h->isoPool, &h->isoCtr, &h->isoStreamCount, &h->isoFirst, &h->isoOrdered};
    for (DevBuf *b: bufs)
       b->release();
    HostBuf *hbufs[] = {&h->hRecs, &h->hExt};
@@ -1448,6 +1453,153 @@ int nfcb200_spectrum(nfcb200_handle *h, const void *samples, int samples_on_devi
       }
    }
    CUDA_TRY(cudaStreamSynchronize(st));
+   return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// ISO 7816 contact smart-card traffic from 4-channel logic captures (lab::IsoDecoder, iso_decode.cuh)
+// ---------------------------------------------------------------------------------------------------------------------
+int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams, uint64_t n_samples,
+                                 uint32_t sample_rate, nfcb200_frame *out, uint64_t cap, uint64_t *n_out)
+{
+   if (!h)
+      return fail(NFCB200_ERR_INVALID, "null handle");
+   if (n_out)
+      *n_out = 0;
+   if (sigtype != NFCB200_SIG_LOGIC_F32 && sigtype != NFCB200_SIG_LOGIC_S16)
+      return fail(NFCB200_ERR_INVALID, "signal type %d is not a 4-channel logic format", sigtype);
+   if (sample_rate == 0)
+      return fail(NFCB200_ERR_INVALID, "sample rate of 0");
+   if (!samples || n_streams == 0 || n_samples == 0)
+      return fail(NFCB200_ERR_INVALID, "empty batch");
+   if (cap && !out)
+      return fail(NFCB200_ERR_INVALID, "null frame buffer");
+   if (n_samples >= 0xFFFFFFFFull)
+      return fail(NFCB200_ERR_UNSUPPORTED, "streams of 2^32 - 1 samples or more exceed the 32-bit sample clock of the reference (IsoTech.h:221)");
+   const bool s16 = sigtype == NFCB200_SIG_LOGIC_S16;
+   const uint64_t bs = s16 ? 8 : 16;
+   if (samples_on_device && ((uintptr_t) samples % bs))
+      return fail(NFCB200_ERR_INVALID, "device samples not aligned to %u bytes", (unsigned) bs);
+
+   CUDA_TRY(cudaSetDevice(h->device));
+   cudaStream_t st = h->stream;
+   int rc;
+
+   // host input is staged a group of whole streams at a time (about 1 GB); a group's streams are the edge pass's grid.y
+   const uint64_t streamBytes = n_samples * bs;
+   const uint64_t maxGroup = samples_on_device ? n_streams : std::max<uint64_t>(1, (1ull << 30) / streamBytes);
+   const uint32_t chunkStreams = (uint32_t) std::min<uint64_t>(std::min<uint64_t>(n_streams, maxGroup), 65535);
+   const uint32_t nTiles = (uint32_t) ((n_samples + ISO_TILE - 1) / ISO_TILE);
+   const uint64_t chunkTiles = (uint64_t) chunkStreams * nTiles;
+   if (!samples_on_device && (rc = h->isoIn.reserve((uint64_t) chunkStreams * streamBytes)))
+      return rc;
+   if ((rc = h->isoClkCount.reserve(chunkTiles * 4)) || (rc = h->isoLineCount.reserve(chunkTiles * 4)) || (rc = h->isoCtr.reserve(8)) ||
+       (rc = h->isoStreamCount.reserve((uint64_t) chunkStreams * 4)) || (rc = h->isoFirst.reserve((uint64_t) chunkStreams * 8)))
+      return rc;
+   uint32_t poolCap = (uint32_t) std::max<uint64_t>(1024, h->isoPool.cap / sizeof(nfcb200_frame));
+   if ((rc = h->isoPool.reserve((uint64_t) poolCap * sizeof(nfcb200_frame))))
+      return rc;
+
+   uint64_t nf = 0; // frames of the chunks so far
+   std::vector<uint32_t> streamCount(chunkStreams);
+   std::vector<uint64_t> first(chunkStreams);
+   for (uint32_t s0 = 0; s0 < n_streams; s0 += chunkStreams)
+   {
+      const uint32_t sc = std::min(chunkStreams, n_streams - s0);
+      IsoEdgesArgs E = {};
+      if (samples_on_device)
+         E.samples = (const unsigned char *) samples + (uint64_t) s0 * streamBytes;
+      else
+      {
+         CUDA_TRY(cudaMemcpyAsync(h->isoIn.ptr, (const unsigned char *) samples + (uint64_t) s0 * streamBytes, (uint64_t) sc * streamBytes,
+                                  cudaMemcpyHostToDevice, st));
+         E.samples = h->isoIn.ptr;
+      }
+      E.n_samples = n_samples;
+      E.n_tiles = nTiles;
+      E.line_count = h->isoLineCount.as<uint32_t>();
+      E.clk_count = h->isoClkCount.as<uint32_t>();
+      E.overflow = h->isoCtr.as<uint32_t>() + 1;
+      // the dense pass, again with room for a line event and a CLK falling edge at every sample when a tile overflows
+      // the first try's slots
+      for (E.line_cap = ISO_LINE_CAP, E.clk_cap = ISO_CLK_CAP;; E.line_cap = E.clk_cap = ISO_TILE)
+      {
+         if ((rc = h->isoLine.reserve((uint64_t) sc * nTiles * E.line_cap * 4)) ||
+             (rc = h->isoClk.reserve((uint64_t) sc * nTiles * E.clk_cap * sizeof(uint16_t))))
+            return rc;
+         E.line = h->isoLine.as<uint32_t>();
+         E.clk = h->isoClk.as<uint16_t>();
+         CUDA_TRY(cudaMemsetAsync(E.overflow, 0, 4, st));
+         const dim3 grid(nTiles, sc);
+         if (s16)
+            iso_edges_kernel<true><<<grid, ISO_THREADS, 0, st>>>(E);
+         else
+            iso_edges_kernel<false><<<grid, ISO_THREADS, 0, st>>>(E);
+         CUDA_TRY(cudaGetLastError());
+         uint32_t overflow = 0;
+         CUDA_TRY(cudaMemcpyAsync(&overflow, E.overflow, 4, cudaMemcpyDeviceToHost, st));
+         CUDA_TRY(cudaStreamSynchronize(st));
+         if (!overflow || E.line_cap == ISO_TILE)
+            break;
+      }
+      // the walk, again with a larger pool when the frames did not fit
+      IsoWalkArgs W = {};
+      W.n_streams = sc;
+      W.stream0 = s0;
+      W.n_samples = (uint32_t) n_samples;
+      W.n_tiles = nTiles;
+      W.line_cap = E.line_cap;
+      W.clk_cap = E.clk_cap;
+      W.sample_rate = sample_rate;
+      W.stream_time = h->cfg.stream_time;
+      W.line = E.line;
+      W.line_count = E.line_count;
+      W.clk = E.clk;
+      W.clk_count = E.clk_count;
+      W.pool_count = h->isoCtr.as<uint32_t>();
+      W.stream_count = h->isoStreamCount.as<uint32_t>();
+      uint32_t count = 0;
+      while (true)
+      {
+         W.pool = h->isoPool.as<nfcb200_frame>();
+         W.pool_cap = poolCap;
+         CUDA_TRY(cudaMemsetAsync(W.pool_count, 0, 4, st));
+         iso_walk_kernel<<<sc, 32, 0, st>>>(W);
+         CUDA_TRY(cudaGetLastError());
+         CUDA_TRY(cudaMemcpyAsync(&count, W.pool_count, 4, cudaMemcpyDeviceToHost, st));
+         CUDA_TRY(cudaStreamSynchronize(st));
+         if (count <= poolCap)
+            break;
+         poolCap = count;
+         if ((rc = h->isoPool.reserve((uint64_t) poolCap * sizeof(nfcb200_frame))))
+            return rc;
+      }
+      // (stream, rank in the stream): the order the reference returns each capture's frames in
+      if (count && nf < cap)
+      {
+         CUDA_TRY(cudaMemcpy(streamCount.data(), W.stream_count, (uint64_t) sc * 4, cudaMemcpyDeviceToHost));
+         uint64_t at = 0;
+         for (uint32_t i = 0; i < sc; i++)
+         {
+            first[i] = at;
+            at += streamCount[i];
+         }
+         if ((rc = h->isoOrdered.reserve((uint64_t) count * sizeof(nfcb200_frame))))
+            return rc;
+         CUDA_TRY(cudaMemcpyAsync(h->isoFirst.ptr, first.data(), (uint64_t) sc * 8, cudaMemcpyHostToDevice, st));
+         const uint32_t blocks = (uint32_t) std::min<uint64_t>((count + 7) / 8, (uint64_t) h->smCount * 16);
+         iso_gather_kernel<<<blocks, 256, 0, st>>>(W.pool, count, h->isoFirst.as<uint64_t>(), s0, h->isoOrdered.as<nfcb200_frame>());
+         CUDA_TRY(cudaGetLastError());
+         CUDA_TRY(cudaMemcpyAsync(out + nf, h->isoOrdered.ptr, std::min<uint64_t>(count, cap - nf) * sizeof(nfcb200_frame), cudaMemcpyDeviceToHost, st));
+         CUDA_TRY(cudaStreamSynchronize(st));
+      }
+      nf += count;
+   }
+
+   if (n_out)
+      *n_out = nf;
+   if (nf > cap)
+      return fail(NFCB200_ERR_CAPACITY, "%llu frames decoded but room for %llu only", (unsigned long long) nf, (unsigned long long) cap);
    return 0;
 }
 

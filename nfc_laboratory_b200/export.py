@@ -11,6 +11,10 @@ Host-side plumbing, no device code:
 A frame is anything with the fields of binding.Frame / include/nfcb200.h: tech_type, frame_type, frame_flags, frame_phase,
 frame_rate, sample_start, sample_end, data -- plus sample_rate and stream_time passed by the caller (time_start =
 double(sample_start) / double(sample_rate), date_time = stream_time + time_start, lab-radio NfcA.cpp:539-547).
+
+ISO 7816 frames (tech 0x0200 / 0x0201, NfcDecoder.iso7816_decode) carry their own date_time: the reference sets it to
+stream_time alone for ATR, T=0 and T=1 frames (Iso7816.cpp:529-530, 618-619, 670-671).  Given a frame record that has a
+date_time field (binding.CFrame, a FRAME_DTYPE record), the writers below use it for those frames.
 """
 import io
 import json
@@ -20,15 +24,23 @@ import tarfile
 FT_CARRIER_OFF, FT_CARRIER_ON, FT_POLL, FT_LISTEN = 0x0100, 0x0101, 0x0102, 0x0103
 FLAG_ENCRYPTED, FLAG_TRUNCATED, FLAG_PARITY, FLAG_CRC, FLAG_SYNC = 0x02, 0x08, 0x10, 0x20, 0x40
 
-FRAME_TYPE_NAMES = {FT_CARRIER_OFF: "CarrierOff", FT_CARRIER_ON: "CarrierOn", FT_POLL: "Poll", FT_LISTEN: "Listen"}
-FRAME_TECH_NAMES = {0x0000: "None", 0x0101: "NfcA", 0x0102: "NfcB", 0x0103: "NfcF", 0x0104: "NfcV"}
+TECH_ISO_ANY, TECH_ISO7816 = 0x0200, 0x0201
+
+FRAME_TYPE_NAMES = {FT_CARRIER_OFF: "CarrierOff", FT_CARRIER_ON: "CarrierOn", FT_POLL: "Poll", FT_LISTEN: "Listen",
+                    0x0200: "VccLow", 0x0201: "VccHigh", 0x0202: "RstLow", 0x0203: "RstHigh",
+                    0x0210: "ATR", 0x0211: "Request", 0x0212: "Response", 0x0213: "Exchange"}
+FRAME_TECH_NAMES = {0x0000: "None", 0x0101: "NfcA", 0x0102: "NfcB", 0x0103: "NfcF", 0x0104: "NfcV",
+                    TECH_ISO_ANY: "IsoAny", TECH_ISO7816: "ISO7816"}
 
 
 def _fields(frame):
-    """(tech, type, flags, phase, rate, start, end, payload) of a binding.Frame, a tuple key, or a FRAME_DTYPE record"""
+    """(tech, type, flags, phase, rate, start, end, payload) of a binding.Frame or CFrame, a tuple key, or a FRAME_DTYPE record"""
     if hasattr(frame, "tech_type"):
+        data = bytes(frame.data)
+        if hasattr(frame, "length"):  # binding.CFrame: the payload is the first `length` bytes of data[512]
+            data = data[: int(frame.length)]
         return (int(frame.tech_type), int(frame.frame_type), int(frame.frame_flags), int(frame.frame_phase), int(frame.frame_rate),
-                int(frame.sample_start), int(frame.sample_end), bytes(frame.data))
+                int(frame.sample_start), int(frame.sample_end), data)
     if hasattr(frame, "dtype") and frame.dtype.names:
         return (int(frame["tech_type"]), int(frame["frame_type"]), int(frame["frame_flags"]), int(frame["frame_phase"]), int(frame["frame_rate"]),
                 int(frame["sample_start"]), int(frame["sample_end"]), bytes(frame["data"][: int(frame["length"])]))
@@ -36,6 +48,16 @@ def _fields(frame):
     if len(t) == 9:  # leading stream index
         t = t[1:]
     return (int(t[0]), int(t[1]), int(t[2]), int(t[3]), int(t[4]), int(t[5]), int(t[6]), bytes(t[7]))
+
+
+def _date_time(frame, tech, stream_time, time_start):
+    """an ISO frame's own date_time when the record has one, else stream_time + time_start"""
+    if tech in (TECH_ISO_ANY, TECH_ISO7816):
+        if hasattr(frame, "date_time"):
+            return float(frame.date_time)
+        if hasattr(frame, "dtype") and frame.dtype.names and "date_time" in frame.dtype.names:
+            return float(frame["date_time"])
+    return float(stream_time) + time_start
 
 
 def trz_entry(frame, sample_rate, stream_time=0.0, range_start=0.0):
@@ -55,7 +77,7 @@ def trz_entry(frame, sample_rate, stream_time=0.0, range_start=0.0):
         "frameRate": rate,
         "frameFlags": flags,
         "framePhase": phase,
-        "dateTime": float(stream_time) + time_start,
+        "dateTime": _date_time(frame, tech, stream_time, time_start),
     }
     if payload:
         e["frameData"] = ":".join("%02X" % b for b in payload)
@@ -109,7 +131,7 @@ def rx_json_line(frame, sample_rate, stream_time=0.0):
     tech, ftype, flags, phase, rate, start, end, payload = _fields(frame)
     time_start = float(start) / float(sample_rate)
     time_end = float(end) / float(sample_rate)
-    date_time = float(stream_time) + time_start
+    date_time = _date_time(frame, tech, stream_time, time_start)
     o = {
         "timestamp": start,
         "tech": FRAME_TECH_NAMES.get(tech, "UNKNOWN"),

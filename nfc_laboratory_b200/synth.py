@@ -415,3 +415,148 @@ def synth_batch(config, n_streams, n_samples, seed=1, device="cpu", fs=10_000_00
             sgm = torch.from_numpy(sg[s0:s1]).to(dev)[:, None]
             out[s0:s1] = (x + sgm * torch.randn(x.shape, generator=gen, device=dev)).abs()
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ISO 7816 contact smart-card captures: 4 logic channels IO, CLK, RST, VCC (the reference's logic capture layout)
+# ---------------------------------------------------------------------------------------------------------------------
+ISO_SCENARIOS = ("t0_direct", "t0_inverse", "t1_lrc", "t1_crc", "warm_reset")
+
+
+def _iso_lrc(data):
+    x = 0
+    for b in data:
+        x ^= b
+    return x
+
+
+class _IsoLine:
+    """a capture under construction: times in seconds, IO as a list of low intervals, an ETU in seconds"""
+
+    def __init__(self, rng, clock_hz, inverse):
+        self.rng = rng
+        self.clock = clock_hz
+        self.inverse = inverse
+        self.etu = 372.0 / clock_hz
+        self.low = []           # IO low intervals (t0, t1)
+        self.t = 0.0
+
+    def char(self, byte, parity_error=False, error_signal=False):
+        """one character from self.t: start bit, 8 data bits, even parity; the receiver's error signal when asked"""
+        bits = [(byte >> i) & 1 for i in (range(7, -1, -1) if self.inverse else range(8))]
+        par = (bin(byte).count("1") & 1) ^ (1 if parity_error else 0)
+        levels = [0] + [(1 - b) if self.inverse else b for b in bits] + [(1 - par) if self.inverse else par]
+        for k, lv in enumerate(levels):
+            if lv == 0:
+                self.low.append((self.t + k * self.etu, self.t + (k + 1) * self.etu))
+        if error_signal:
+            self.low.append((self.t + 10.2 * self.etu, self.t + 11.7 * self.etu))
+            self.t += 14 * self.etu
+        else:
+            self.t += (12 + self.rng.uniform(0.0, 0.6)) * self.etu
+
+    def frame(self, data, gap_etu=20.0, bad=None):
+        """bytes back to back; index `bad` goes out once with a parity error, is refused and repeated"""
+        for i, b in enumerate(data):
+            if i == bad:
+                self.char(b, parity_error=True, error_signal=True)
+            self.char(b)
+        self.t += gap_etu * self.etu
+
+
+def iso7816_capture(scenario, rate, seed=1, glitches=True):
+    """one seeded capture [n, 4] float32 (IO, CLK, RST, VCC as 0 / 1): power-up, clock, reset, ATR and an exchange.
+
+    t0_direct   direct-convention ATR, PPS to Fi 1 / Di 3, T=0 TPDUs with NULL and ACK procedure bytes, one character
+                with a parity error that the receiver signals and the sender repeats, a clock change of more than 5 %
+    t0_inverse  the same in the inverse convention
+    t1_lrc      ATR announcing T=1, PPS to T=1, I / R / S blocks with an LRC epilogue
+    t1_crc      the same blocks with a CRC epilogue (the reference decodes with the LRC rule: its ATR parser never
+                selects CRC)
+    warm_reset  a T=0 session, RST low mid-capture, a second ATR
+    Every capture ends with power-off.  `glitches` adds one-sample pulses on IO (before the reset) and on CLK."""
+    rng = np.random.default_rng(seed)
+    clock1 = float(rng.choice([3.5712e6, 4.0e6, 2.5e6]))
+    clock2 = clock1 * float(rng.choice([0.85, 1.12]))
+    line = _IsoLine(rng, clock1, scenario == "t0_inverse")
+    t_vcc = 20e-6
+    t_clk = t_vcc + 5e-6
+    t_rst = t_clk + 500 / clock1
+    line.t = t_rst + 600 / clock1
+    t_chg = None
+    rst_low = []
+
+    if scenario.startswith("t1"):
+        atr = [0x3B, 0x91, 0x13, 0x81, 0x31, 0xFE, 0x45, 0x4A]      # TA1 TD1(T=1) TD2 TA3(IFSC) TB3(BWI/CWI) + 1 hist
+        atr.append(_iso_lrc(atr[1:]))
+    elif scenario == "t0_inverse":
+        atr = [0x3F, 0x12, 0x11, 0x41, 0x42]
+    else:
+        atr = [0x3B, 0x12, 0x11, 0x41, 0x42]
+    line.frame(atr, gap_etu=200)
+
+    t1 = scenario.startswith("t1")
+    pps = [0xFF, 0x11 if t1 else 0x10, 0x13]
+    pps.append(_iso_lrc(pps))
+    line.frame(pps, gap_etu=30)
+    line.frame(pps, gap_etu=100)
+    line.etu = 372.0 / 4 / line.clock
+
+    if t1:
+        crc = scenario == "t1_crc"
+
+        def block(nad, pcb, inf):
+            b = [nad, pcb, len(inf)] + list(inf)
+            if crc:
+                c = _crc16_refl(b, 0xFFFF) ^ 0xFFFF
+                return b + [c & 0xFF, c >> 8]
+            return b + [_iso_lrc(b)]
+
+        for blk in (block(0x00, 0x00, [0x00, 0xA4, 0x04, 0x00]), block(0x00, 0x00, [0x90, 0x00]),
+                    block(0x00, 0x91, []), block(0x00, 0xC1, [0xFE]), block(0x00, 0xE1, [0xFE]),
+                    block(0x00, 0x40, [0x00, 0xB0, 0x00, 0x00, 0x04]), block(0x00, 0x40, [0x01, 0x02, 0x03, 0x04, 0x90, 0x00])):
+            line.frame(blk, gap_etu=80)
+        t_chg = line.t
+        line.clock = clock2
+        line.etu = 372.0 / 4 / clock2
+        line.t += 400 * line.etu
+        line.frame(block(0x00, 0x00, [0x00, 0x84, 0x00, 0x00, 0x08]), gap_etu=80)
+    else:
+        # SELECT with an ACK procedure byte, one character repeated after a parity error
+        line.frame([0x00, 0xA4, 0x04, 0x00, 0x02, 0xA4, 0x3F, 0x00, 0x90, 0x00], gap_etu=40, bad=6)
+        # GET CHALLENGE with a NULL procedure byte, then per-byte ACKs (INS ^ 0xFF)
+        line.frame([0x00, 0x84, 0x00, 0x00, 0x02, 0x60, 0x84, 0x11, 0x22, 0x90, 0x00], gap_etu=40)
+        line.frame([0x80, 0xCA, 0x9F, 0x7F, 0x01, 0x35, 0x55, 0x61, 0x05], gap_etu=40)
+        t_chg = line.t
+        line.clock = clock2
+        line.etu = 372.0 / 4 / clock2
+        line.t += 400 * line.etu
+        line.frame([0x00, 0xB0, 0x00, 0x00, 0x02, 0xB0, 0xAA, 0xBB, 0x90, 0x00], gap_etu=200)
+        if scenario == "warm_reset":
+            rst_low.append((line.t, line.t + 300 / line.clock))
+            line.t += 300 / line.clock + 600 / line.clock
+            line.etu = 372.0 / line.clock
+            line.frame([0x3B, 0x00], gap_etu=100)
+            line.frame([0x00, 0xA4, 0x04, 0x00, 0x02, 0xA4, 0x3F, 0x00, 0x90, 0x00], gap_etu=100)
+
+    t_off = line.t + 100e-6
+    n = int((t_off + 30e-6) * rate)
+    t = np.arange(n, dtype=np.float64) / rate
+    vcc = ((t >= t_vcc) & (t < t_off)).astype(np.float32)
+    rst = ((t >= t_rst) & (t < t_off)).astype(np.float32)
+    for a, b in rst_low:
+        rst[(t >= a) & (t < b)] = 0
+    phase = np.where(t < t_chg, (t - t_clk) * clock1, (t_chg - t_clk) * clock1 + (t - t_chg) * clock2)
+    clk = (((phase % 1.0) < 0.5) & (t >= t_clk) & (t < t_off - 10e-6)).astype(np.float32)
+    io = ((t >= t_vcc + 2e-6) & (t < t_off)).astype(np.float32)
+    for a, b in line.low:
+        io[(t >= a) & (t < b)] = 0
+    if glitches:
+        # IO glitches before the reset: a glitch inside a T=0 session starts a character that swallows the session
+        # (a frame then ends only after CWT = 9600 ETU)
+        idle = np.flatnonzero((io[1:-1] == 1) & (io[:-2] == 1) & (io[2:] == 1) & (t[1:-1] < t_rst)) + 1
+        for i in rng.choice(idle, size=min(3, idle.size), replace=False):
+            io[i] = 0
+        for i in rng.integers(int(t_clk * rate) + 10, n - 10, size=3):
+            clk[i] = 1 - clk[i]
+    return np.stack([io, clk, rst, vcc], axis=1)
