@@ -254,18 +254,46 @@ class NfcDecoder:
                               int(f.sample_start), int(f.sample_end), bytes(f.data[:f.length]))))
         return out
 
-    def decode_batch_ptr(self, ptr, on_device, sigtype, n_streams, n_samples, sample_rate, cap=1 << 16, raw=False):
-        """decode [n_streams][n_samples] samples at `ptr` (host or device address)"""
+    def _with_room(self, call, cap, raw):
+        """call(buf, cap, byref(n)) of a C entry point that returns frames, again with room for all of them when the first
+        buffer was too small"""
         while True:
             buf = self._buffer(cap)
             n = C.c_uint64(0)
-            rc = self._lib.nfcb200_decode_batch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams, n_samples,
-                                                sample_rate, buf, cap, C.byref(n))
+            rc = call(buf, cap, C.byref(n))
             if rc == -4 and n.value > cap:
                 cap = int(n.value) + 16
                 continue
             _check(self._lib, rc)
             return (buf, n.value) if raw else self._convert(buf, n.value)
+
+    def _batch(self, samples, sigtype):
+        """(array, address, on_device) of a batch [n_streams, n_samples(, components)], or of one stream without the first
+        axis, made contiguous: a numpy array is converted to the signal type's dtype; a torch tensor must have that dtype
+        and lie on the host or on this decoder's device.  The library reads a CUDA tensor on its own stream, so torch's
+        current stream is waited for first."""
+        dtype, comps = _SIG_DTYPE[sigtype]
+        one_stream = 1 if comps == 1 else 2
+        if isinstance(samples, np.ndarray):
+            a = np.ascontiguousarray(samples, dtype=dtype)
+            a = a[None] if a.ndim == one_stream else a
+            return a, a.ctypes.data, False
+        import torch
+        if samples.is_cuda and samples.device.index != self._cfg.device:
+            raise NfcB200Error(-2, "tensor on %s, decoder on cuda:%d" % (samples.device, self._cfg.device))
+        want = torch.float32 if dtype == np.float32 else torch.int16
+        if samples.dtype != want:
+            raise NfcB200Error(-2, "signal type %d takes %s samples, got a %s tensor" % (sigtype, want, samples.dtype))
+        t = samples.contiguous()
+        t = t[None] if t.dim() == one_stream else t
+        if t.is_cuda:
+            torch.cuda.current_stream(t.device).synchronize()
+        return t, t.data_ptr(), t.is_cuda
+
+    def decode_batch_ptr(self, ptr, on_device, sigtype, n_streams, n_samples, sample_rate, cap=1 << 16, raw=False):
+        """decode [n_streams][n_samples] samples at `ptr` (host or device address)"""
+        return self._with_room(lambda buf, cap, n: self._lib.nfcb200_decode_batch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams,
+                                                                               n_samples, sample_rate, buf, cap, n), cap, raw)
 
     def set_carry(self, blob, clock_shift=0):
         """carry in front of the next single-stream decode (a time shard continuing a capture); None clears"""
@@ -311,45 +339,23 @@ class NfcDecoder:
         return (buf, int(n.value)) if raw else self._convert(buf, int(n.value))
 
     def decode_batch(self, samples, sigtype, sample_rate, cap=1 << 16):
-        """samples: numpy array [n_streams, n_samples(, 2)] or torch CUDA tensor of the same shape"""
-        dtype, comps = _SIG_DTYPE[sigtype]
-        if isinstance(samples, np.ndarray):
-            a = np.ascontiguousarray(samples, dtype=dtype)
-            if a.ndim == (1 if comps == 1 else 2):
-                a = a[None]
-            n_streams, n_samples = a.shape[0], a.shape[1]
-            return self.decode_batch_ptr(a.ctypes.data, False, sigtype, n_streams, n_samples, sample_rate, cap)
-        # torch tensor
-        t = samples.contiguous()
-        if t.dim() == (1 if comps == 1 else 2):
-            t = t[None]
-        n_streams, n_samples = t.shape[0], t.shape[1]
-        return self.decode_batch_ptr(t.data_ptr(), t.is_cuda, sigtype, n_streams, n_samples, sample_rate, cap)
+        """samples: numpy array [n_streams, n_samples(, 2)] or torch tensor of the same shape"""
+        a, ptr, on_device = self._batch(samples, sigtype)
+        return self.decode_batch_ptr(ptr, on_device, sigtype, int(a.shape[0]), int(a.shape[1]), sample_rate, cap)
 
     def spectrum(self, samples, sigtype, sample_rate, hop=None):
         """FFT spectrum of the reference's frequency view (lab::FourierProcessTask) every `hop` samples of every stream
         (hop=None: one frame per span of 1024 x decimation samples).  samples: IQ as numpy [n_streams, n_samples, 2] (or one
         stream [n_samples, 2]) -> numpy float32 [n_streams, frames, 1024]; a CUDA tensor of the same shape -> a CUDA tensor
         on the same device.  Bins run from the most negative frequency up (include/nfcb200.h nfcb200_spectrum)."""
-        dtype, comps = _SIG_DTYPE[sigtype]
-        if isinstance(samples, np.ndarray):
-            a = np.ascontiguousarray(samples, dtype=dtype)
-            a = a[None] if a.ndim == comps else a
-            ptr, on_device = a.ctypes.data, False
-        else:
-            import torch
-            a = samples.contiguous()
-            a = a[None] if a.dim() == comps else a
-            if a.is_cuda and a.device.index != self._cfg.device:
-                raise NfcB200Error(-2, "tensor on %s, decoder on cuda:%d" % (a.device, self._cfg.device))
-            ptr, on_device = a.data_ptr(), a.is_cuda
+        a, ptr, on_device = self._batch(samples, sigtype)
         n_streams, n_samples = int(a.shape[0]), int(a.shape[1])
         if hop is None:
             hop = SPECTRUM_BINS * spectrum_shape(n_samples, sample_rate)[1]
         n_frames = spectrum_shape(n_samples, sample_rate, hop)[0]
         if on_device:
+            import torch
             out = torch.empty((n_streams, n_frames, SPECTRUM_BINS), dtype=torch.float32, device=a.device)
-            torch.cuda.current_stream(a.device).synchronize()  # the library's stream does not wait for torch's
             self.spectrum_ptr(ptr, True, sigtype, n_streams, n_samples, sample_rate, hop, out.data_ptr(), True, out.numel())
         else:
             out = np.empty((n_streams, n_frames, SPECTRUM_BINS), dtype=np.float32)
@@ -368,39 +374,14 @@ class NfcDecoder:
         [n_streams, n_samples, 4] (or one stream [n_samples, 4]), float32 for SIG_LOGIC_F32 or int16 for SIG_LOGIC_S16, or a
         torch tensor of the same shape (a CUDA tensor is decoded where it lies).  Frames are ordered by (stream, time).
         raw=True returns (CFrame buffer, count) with every field, time_start / time_end / date_time included."""
-        dtype, comps = _SIG_DTYPE[sigtype]
-        if comps != 4:
+        if _SIG_DTYPE[sigtype][1] != 4:
             raise NfcB200Error(-2, "signal type %d is not a 4-channel logic format" % sigtype)
-        keep = None
-        if isinstance(samples, np.ndarray):
-            a = np.ascontiguousarray(samples, dtype=dtype)
-            a = a[None] if a.ndim == 2 else a
-            ptr, on_device, keep = a.ctypes.data, False, a
-        else:
-            import torch
-            a = samples.contiguous()
-            a = a[None] if a.dim() == 2 else a
-            if a.is_cuda and a.device.index != self._cfg.device:
-                raise NfcB200Error(-2, "tensor on %s, decoder on cuda:%d" % (a.device, self._cfg.device))
-            want = torch.float32 if dtype == np.float32 else torch.int16
-            if a.dtype != want:
-                raise NfcB200Error(-2, "signal type %d takes %s samples, got a %s tensor" % (sigtype, want, a.dtype))
-            if a.is_cuda:
-                torch.cuda.current_stream(a.device).synchronize()  # the library's stream does not wait for torch's
-            ptr, on_device, keep = a.data_ptr(), a.is_cuda, a
-        if len(keep.shape) != 3 or keep.shape[2] != 4:
-            raise NfcB200Error(-2, "logic samples must be [n_streams, n_samples, 4], got %s" % (tuple(keep.shape),))
-        n_streams, n_samples = int(keep.shape[0]), int(keep.shape[1])
-        while True:
-            buf = self._buffer(cap)
-            n = C.c_uint64(0)
-            rc = self._lib.nfcb200_iso7816_decode_batch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams, n_samples,
-                                                        int(sample_rate), buf, cap, C.byref(n))
-            if rc == -4 and n.value > cap:
-                cap = int(n.value) + 16
-                continue
-            _check(self._lib, rc)
-            return (buf, n.value) if raw else self._convert(buf, n.value)
+        a, ptr, on_device = self._batch(samples, sigtype)
+        if len(a.shape) != 3 or a.shape[2] != 4:
+            raise NfcB200Error(-2, "logic samples must be [n_streams, n_samples, 4], got %s" % (tuple(a.shape),))
+        n_streams, n_samples = int(a.shape[0]), int(a.shape[1])
+        return self._with_room(lambda buf, cap, n: self._lib.nfcb200_iso7816_decode_batch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype,
+                                                                                       n_streams, n_samples, int(sample_rate), buf, cap, n), cap, raw)
 
     def nextFrames(self, samples, sample_rate=None, sigtype=SIG_MAG_F32, cap=4096):
         """NfcDecoder::nextFrames(SignalBuffer): streaming decode of one capture.  samples=None (an invalid buffer in the
