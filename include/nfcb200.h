@@ -248,6 +248,28 @@ int nfcb200_spectrum_shape(uint64_t n_samples, uint32_t sample_rate, uint64_t ho
 int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams, uint64_t n_samples,
                                  uint32_t sample_rate, nfcb200_frame *out, uint64_t cap, uint64_t *n_out);
 
+/*
+ * Streaming ISO 7816 decode of ONE logic capture in arbitrary buffers: replaces lab::IsoDecoder::nextFrames(SignalBuffer)
+ * called per buffer by LogicDecoderTask (LogicDecoderTask.cpp:300), and nextFrames({}) on stop (:186, :261).  Input is
+ * host memory, n samples of 4 channels in `sigtype` format (NFCB200_SIG_LOGIC_F32 or NFCB200_SIG_LOGIC_S16).  The decoder
+ * state, the last sample included, carries from buffer to buffer, and so does the reference's call boundary: a buffer
+ * picks its loop afresh (detect unless an ATR locked the protocol), so where buffers end can change the frames, as it does
+ * in the reference (DESIGN.md section 13).  A buffer at another sample rate restarts the sample clock at 0 and resets the
+ * protocol.  date_time uses config.stream_time as it is at the push.  n == 0 is nextFrames({}): it decodes nothing and
+ * delivers what is pending.  More frames than cap: NFCB200_ERR_CAPACITY after delivering cap, the rest wait in
+ * nfcb200_iso7816_stream_pending (nothing is lost).  A stream whose sample clock would pass 2^32 - 1 samples is refused
+ * with NFCB200_ERR_UNSUPPORTED.  The ISO stream leaves every other state of the handle alone (NFC stream, batch decode
+ * state, spectrum, ISO batch), and they leave it alone.
+ */
+int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *samples, int sigtype, uint64_t n, uint32_t sample_rate, nfcb200_frame *out,
+                                uint64_t cap, uint64_t *n_out);
+
+/* frames of the ISO stream that did not fit an earlier push's buffer: up to cap of them, *n_left = how many remain */
+int nfcb200_iso7816_stream_pending(nfcb200_handle *h, nfcb200_frame *out, uint64_t cap, uint64_t *n_out, uint64_t *n_left);
+
+/* forget the ISO stream: the next push decodes as on a fresh handle (the sample before it is 0) */
+int nfcb200_iso7816_stream_reset(nfcb200_handle *h);
+
 const char *nfcb200_last_error(void);
 
 /* library / build identification, e.g. "nfcb200 0.1 sm_90a" */

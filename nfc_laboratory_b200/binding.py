@@ -128,6 +128,10 @@ def load_library():
                                      C.c_uint64, C.POINTER(C.c_uint64)]
     lib.nfcb200_iso7816_decode_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint32, C.c_uint64, C.c_uint32,
                                                  C.POINTER(CFrame), C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.nfcb200_iso7816_stream_push.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.POINTER(CFrame), C.c_uint64,
+                                                C.POINTER(C.c_uint64)]
+    lib.nfcb200_iso7816_stream_pending.argtypes = [C.c_void_p, C.POINTER(CFrame), C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    lib.nfcb200_iso7816_stream_reset.argtypes = [C.c_void_p]
     lib.nfcb200_spectrum_shape.argtypes = [C.c_uint64, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
     _lib = lib
     return lib
@@ -382,6 +386,43 @@ class NfcDecoder:
         n_streams, n_samples = int(a.shape[0]), int(a.shape[1])
         return self._with_room(lambda buf, cap, n: self._lib.nfcb200_iso7816_decode_batch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype,
                                                                                        n_streams, n_samples, int(sample_rate), buf, cap, n), cap, raw)
+
+    def iso7816_push(self, samples, sigtype, sample_rate, cap=4096, raw=False):
+        """lab::IsoDecoder::nextFrames(SignalBuffer) of one buffer of a live logic capture [n_samples, 4] (numpy, float32 for
+        SIG_LOGIC_F32 or int16 for SIG_LOGIC_S16): the frames it completes, every pending one included.  The decoder carries
+        over to the next push; a push at another sample rate restarts it.  Frames as iso7816_decode returns them; raw=True
+        gives a list of CFrame with every field."""
+        if _SIG_DTYPE.get(sigtype, (None, 0))[1] != 4:
+            raise NfcB200Error(-2, "signal type %d is not a 4-channel logic format" % sigtype)
+        a = np.ascontiguousarray(samples, dtype=_SIG_DTYPE[sigtype][0])
+        if a.ndim != 2 or a.shape[1] != 4:
+            raise NfcB200Error(-2, "logic samples must be [n_samples, 4], got %s" % (a.shape,))
+        if a.shape[0] == 0:
+            return self.iso7816_flush(cap, raw)
+        return self._iso_stream(lambda buf, cap, n: self._lib.nfcb200_iso7816_stream_push(self._h, a.ctypes.data, sigtype, a.shape[0], int(sample_rate),
+                                                                                          buf, cap, n), cap, raw)
+
+    def iso7816_flush(self, cap=4096, raw=False):
+        """nextFrames({}) on the ISO stream: it decodes nothing (IsoTech.cpp:31-32); frames still pending are returned"""
+        return self._iso_stream(lambda buf, cap, n: self._lib.nfcb200_iso7816_stream_push(self._h, None, SIG_LOGIC_F32, 0, 0, buf, cap, n), cap, raw)
+
+    def iso7816_reset(self):
+        """forget the ISO stream: the next push decodes as on a fresh decoder"""
+        _check(self._lib, self._lib.nfcb200_iso7816_stream_reset(self._h))
+
+    def _iso_stream(self, call, cap, raw):
+        """call(buf, cap, byref(n)) of an ISO stream push, then its pending frames until none is left"""
+        buf = (CFrame * cap)()
+        n = C.c_uint64(0)
+        rc = call(buf, cap, C.byref(n))
+        if rc != -4:
+            _check(self._lib, rc)
+        frames = [CFrame.from_buffer_copy(f) for f in buf[:n.value]] if raw else self._convert(buf, n.value)
+        left = C.c_uint64(1 if rc == -4 else 0)
+        while left.value:
+            _check(self._lib, self._lib.nfcb200_iso7816_stream_pending(self._h, buf, cap, C.byref(n), C.byref(left)))
+            frames += [CFrame.from_buffer_copy(f) for f in buf[:n.value]] if raw else self._convert(buf, n.value)
+        return frames
 
     def nextFrames(self, samples, sample_rate=None, sigtype=SIG_MAG_F32, cap=4096):
         """NfcDecoder::nextFrames(SignalBuffer): streaming decode of one capture.  samples=None (an invalid buffer in the

@@ -235,11 +235,31 @@ struct nfcb200_handle
       bool tablesReady = false;
    } spec;
 
+   // the ISO 7816 dense pass's per-tile event slots and counts (iso_decode.cuh)
+   struct IsoEvents
+   {
+      nfcb200::DevBuf line, lineCount, clk, clkCount;
+   };
+
    // nfcb200_iso7816_decode_batch: its own buffers too
    struct Iso
    {
-      nfcb200::DevBuf in, line, lineCount, clk, clkCount, pool, ctr, streamCount, first, ordered;
+      IsoEvents ev;
+      nfcb200::DevBuf in, pool, ctr, streamCount, first, ordered;
    } iso;
+
+   // nfcb200_iso7816_stream_push: one live logic capture, beside (not instead of) the NFC stream
+   struct IsoStream
+   {
+      IsoEvents ev;
+      nfcb200::DevBuf in, pool, ctr, streamCount, state; // state: two iso7816::IsoStreamState, the current one is `cur`
+      int cur = 0;
+      bool init = false;                 // a buffer was pushed since the last reset
+      nfcb200::u32 rate = 0;             // sample rate of the last buffer
+      nfcb200::u32 clock = 0;            // samples since the decoder last (re)started: the next buffer's first sample
+      float last[4] = {0, 0, 0, 0};      // the last sample pushed (IsoDecoderStatus::sampleLast), 0 before the first
+      std::vector<nfcb200_frame> pending; // decoded but not yet delivered
+   } isoStream;
 };
 
 #endif

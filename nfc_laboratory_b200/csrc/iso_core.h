@@ -976,6 +976,52 @@ ISO_HD void iso_init(IsoMachine &m, uint32_t sampleRate, uint32_t streamTime)
    m.s.loop = LOOP_DETECT;
 }
 
+// where iso_walk() stops at the end of one buffer of a capture and picks up at the next: the walk's own locals.  CLK falling
+// edges passed since the last step are in clockCounter already (none of them was the 10th, or the walk would have stepped
+// there), so only these two are left
+struct IsoCarry
+{
+   uint64_t wake;   // next sample where a step without edges may act (absolute); ~0 when no timer is pending
+   uint32_t levels; // F_IO_HIGH / F_VCC_HIGH of the last sample (the sample before the first is 0)
+   uint32_t unused;
+};
+
+ISO_HD IsoCarry iso_carry_init()
+{
+   return IsoCarry {~0ull, 0, 0};
+}
+
+// a decoder between two buffers of one capture
+struct IsoStreamState
+{
+   IsoMachine m;
+   IsoCarry c;
+};
+
+// the start of a later nextFrames() call at the same sample rate (IsoDecoder.cpp:184-200): its loop is chosen afresh --
+// detect unless an ATR locked the protocol (`if (!decoder.bitrate)`), then decode()'s switch on the protocol type -- so a
+// buffer that ends inside decodeStreamT0 after a reset cleared the protocol (IsoState::loop) resumes in detect.  A changed
+// loop is a changed state: the first sample of the buffer is stepped.
+ISO_HD void iso_resume(IsoMachine &m, IsoCarry &c, uint32_t base)
+{
+   const uint32_t p = m.s.protocolType;
+   const uint32_t loop = m.s.locked ? (p == 0 ? LOOP_T0 : p == 1 ? LOOP_T1 : LOOP_TX) : LOOP_DETECT;
+   if (loop != m.s.loop)
+   {
+      m.s.loop = loop;
+      c.wake = base < c.wake ? base : c.wake;
+   }
+}
+
+// a buffer at another sample rate (IsoDecoder.cpp:172-178 -> initialize(), :123-156): the clock restarts at 0 and
+// Iso7816::initialize's resetModulation clears every status the machine holds; the last sample survives (IsoTech.cpp:43
+// never reloads it), and with it the levels
+ISO_HD void iso_restart(IsoMachine &m, IsoCarry &c, uint32_t sampleRate, uint32_t streamTime)
+{
+   iso_init(m, sampleRate, streamTime);
+   c.wake = ~0ull;
+}
+
 // earliest timer after `t` (NONE when there is none)
 ISO_HD uint64_t next_timer(const IsoState &s, uint32_t t)
 {
@@ -987,24 +1033,26 @@ ISO_HD uint64_t next_timer(const IsoState &s, uint32_t t)
 }
 
 /*
- * Walk one capture of n samples.  Ev supplies the events in sample order:
+ * Walk one capture, or one buffer of it, up to the sample `end` (absolute: a buffer's first sample is the number of samples
+ * before it since the last (re)start).  Ev supplies the events in sample order, at absolute samples:
  *   line_peek()        sample of the next line event (IO / RST / VCC edge) or NONE;  line_pop() its flags
  *   clk_nth(k)         sample of the k-th (from 0) CLK falling edge not yet consumed, or NONE;  clk_pop() consumes one,
  *                      clk_skip(k) consumes k
- * CLK falling edges are consumed as the walk passes them.
+ * CLK falling edges are consumed as the walk passes them.  `c` holds the walk's state from the end of the previous buffer
+ * and receives it at the end of this one.
  */
 template <class Ev, class Sink>
-ISO_HD void iso_walk(IsoMachine &m, Ev &ev, uint32_t n, Sink &sink)
+ISO_HD void iso_walk(IsoMachine &m, IsoCarry &c, Ev &ev, uint32_t end, Sink &sink)
 {
-   uint32_t levels = 0;  // IO / VCC above 0 since the last line event (the sample before the first is 0)
-   uint64_t wake = ~0ull; // next sample where a step without edges may act
+   uint32_t levels = c.levels; // IO / VCC above 0 since the last line event
+   uint64_t wake = c.wake;     // next sample where a step without edges may act
    while (true)
    {
       const uint64_t tl = ev.line_peek();
       const uint64_t tc = ev.clk_nth(9 - m.clockCounter);
       uint64_t t = tl < tc ? tl : tc;
       t = wake < t ? wake : t;
-      if (t >= n)
+      if (t >= end)
          break;
 #ifdef __CUDA_ARCH__
       // on the device the walk runs on a whole warp, every lane with the same state: clock measurements that only update
@@ -1022,7 +1070,7 @@ ISO_HD void iso_walk(IsoMachine &m, Ev &ev, uint32_t n, Sink &sink)
          const double P = m.s.clockFrequency;
          const bool acts = fabs(v - vprev) / vprev < 0.05 && P > 0 && fabs(v - P) / P > 0.05;
          const uint64_t limit = tl < wake ? tl : wake;
-         const uint32_t stop = __ballot_sync(~0u, acts || tj >= limit || tj >= n);
+         const uint32_t stop = __ballot_sync(~0u, acts || tj >= limit || tj >= end);
          const uint32_t take = stop ? __ffs(stop) - 1 : 32;
          if (take > 0)
          {
@@ -1056,6 +1104,22 @@ ISO_HD void iso_walk(IsoMachine &m, Ev &ev, uint32_t n, Sink &sink)
       st.run();
       wake = state_equal(before, m.s) ? next_timer(m.s, (uint32_t) t) : t + 1;
    }
+   // CLK falling edges between the last step and the end only count
+   while (ev.clk_nth(0) < end)
+   {
+      ev.clk_pop();
+      m.clockCounter++;
+   }
+   c.levels = levels;
+   c.wake = wake;
+}
+
+// a whole capture from its first sample
+template <class Ev, class Sink>
+ISO_HD void iso_walk(IsoMachine &m, Ev &ev, uint32_t n, Sink &sink)
+{
+   IsoCarry c = iso_carry_init();
+   iso_walk(m, c, ev, n, sink);
 }
 
 } // namespace iso7816

@@ -11,7 +11,8 @@
  *                          (noise, a staircase, a ramp) can fall on every sample.
  *   iso_walk_kernel        one warp per stream runs iso_walk() over the tiles' events in order (the lanes evaluate 32
  *                          clock measurements at a time) and appends its frames to a pool with the stream index and the
- *                          frame's rank in its stream, and the stream's frame count.
+ *                          frame's rank in its stream, and the stream's frame count.  A stream pushed buffer by buffer
+ *                          (nfcb200_iso7816_stream_push) resumes from the decoder state the previous buffer left.
  *   iso_gather_kernel      moves every pooled frame to its place in (stream, rank) order: the host's scan of the
  *                          streams' counts gives each stream's first place.
  */
@@ -42,6 +43,8 @@ struct IsoEdgesArgs
    uint16_t *clk;        // [stream][tile][clk_cap]
    uint32_t *clk_count;  // [stream][tile]
    uint32_t *overflow;   // set when a tile has more line events than line_cap or more CLK falling edges than clk_cap
+   float4 last;          // the sample before each stream's first: 0 in a batch (DESIGN.md section 13), the previous
+                         // buffer's last sample in a pushed stream
 };
 
 template <bool S16>
@@ -82,7 +85,7 @@ __global__ void __launch_bounds__(ISO_THREADS) iso_edges_kernel(const IsoEdgesAr
    for (uint32_t j = 0; j < ISO_PER_THREAD; j++)
    {
       const uint64_t i = t0 + j * ISO_THREADS + threadIdx.x;
-      float d[4] = {0, 0, 0, 0}, l[4] = {0, 0, 0, 0};
+      float d[4] = {0, 0, 0, 0}, l[4] = {a.last.x, a.last.y, a.last.z, a.last.w};
       if (i < a.n_samples)
       {
          iso_load<S16>(base, i, d);
@@ -169,13 +172,13 @@ __global__ void __launch_bounds__(ISO_THREADS) iso_edges_kernel(const IsoEdgesAr
    }
 }
 
-// the event source of iso_walk(): the per-tile slots of one stream, read in tile order
+// the event source of iso_walk(): the per-tile slots of one stream, read in tile order, at absolute samples from `base`
 struct IsoDevEvents
 {
    const uint32_t *line, *lineCount;
    const uint16_t *clk;
    const uint32_t *clkCount;
-   uint32_t nTiles, lineCap, clkCap;
+   uint32_t nTiles, lineCap, clkCap, base;
    uint32_t lt = 0, li = 0, ct = 0, ci = 0;
 
    __device__ uint32_t line_peek()
@@ -185,7 +188,7 @@ struct IsoDevEvents
          lt++;
          li = 0;
       }
-      return lt < nTiles ? lt * ISO_TILE + (line[(uint64_t) lt * lineCap + li] & (ISO_TILE - 1)) : iso7816::NONE;
+      return lt < nTiles ? base + lt * ISO_TILE + (line[(uint64_t) lt * lineCap + li] & (ISO_TILE - 1)) : iso7816::NONE;
    }
 
    __device__ uint32_t line_pop()
@@ -202,7 +205,7 @@ struct IsoDevEvents
          if (i < n)
          {
             if (k < n - i)
-               return t * ISO_TILE + clk[(uint64_t) t * clkCap + i + k];
+               return base + t * ISO_TILE + clk[(uint64_t) t * clkCap + i + k];
             k -= n - i;
          }
          t++;
@@ -242,6 +245,11 @@ struct IsoWalkArgs
    uint32_t pool_cap;
    uint32_t *pool_count;
    uint32_t *stream_count; // [n_streams] frames of each stream
+   // a pushed stream (one): the decoder left by the previous buffer, where this buffer's end state goes, the buffer's first
+   // sample and whether its sample rate restarts the decoder.  Unused in a batch: every stream starts fresh at sample 0.
+   const iso7816::IsoStreamState *resume;
+   iso7816::IsoStreamState *state_out;
+   uint32_t base, restart;
 };
 
 struct IsoDevSink
@@ -278,7 +286,9 @@ struct IsoDevSink
    }
 };
 
-// one warp per stream: every lane keeps the same state (iso_walk evaluates clock measurements across the lanes)
+// one warp per stream: every lane keeps the same state (iso_walk evaluates clock measurements across the lanes).  RESUME:
+// a pushed stream, which starts from a.resume and stores its end state (the batch's instance has no such code)
+template <bool RESUME>
 __global__ void __launch_bounds__(32) iso_walk_kernel(const IsoWalkArgs a)
 {
    const uint32_t s = blockIdx.x;
@@ -290,12 +300,35 @@ __global__ void __launch_bounds__(32) iso_walk_kernel(const IsoWalkArgs a)
    ev.nTiles = a.n_tiles;
    ev.lineCap = a.line_cap;
    ev.clkCap = a.clk_cap;
+   ev.base = a.base;
    IsoDevSink sink {&a, a.stream0 + s, 0};
    iso7816::IsoMachine m;
-   iso7816::iso_init(m, a.sample_rate, a.stream_time);
-   iso7816::iso_walk(m, ev, a.n_samples, sink);
+   iso7816::IsoCarry c;
+   if (RESUME)
+   {
+      m = a.resume->m;
+      c = a.resume->c;
+      if (a.restart)
+         iso7816::iso_restart(m, c, a.sample_rate, a.stream_time);
+      else
+         iso7816::iso_resume(m, c, a.base);
+      m.streamTime = a.stream_time;
+   }
+   else
+   {
+      iso7816::iso_init(m, a.sample_rate, a.stream_time);
+      c = iso7816::iso_carry_init();
+   }
+   iso7816::iso_walk(m, c, ev, a.base + a.n_samples, sink);
    if (threadIdx.x == 0)
+   {
       a.stream_count[s] = sink.rank;
+      if (RESUME)
+      {
+         a.state_out->m = m;
+         a.state_out->c = c;
+      }
+   }
 }
 
 // pooled frame k -> out[first[stream - stream0] + rank], the rank field cleared; first[] counts from the chunk's first frame
