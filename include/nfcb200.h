@@ -40,7 +40,9 @@ typedef enum nfcb200_sigtype
    NFCB200_SIG_MAG_S16 = 3,  /* mono int16 PCM                                                                       */
    NFCB200_SIG_IQ_S16 = 4,   /* interleaved int16 I,Q                                                                */
    NFCB200_SIG_LOGIC_F32 = 5,/* SIGNAL_TYPE_LOGIC_SAMPLES, stride 4: float32 IO, CLK, RST, VCC (IsoDecoder input)   */
-   NFCB200_SIG_LOGIC_S16 = 6 /* the same 4 channels as int16 (4-channel 16-bit WAV), read as s / 32768.f              */
+   NFCB200_SIG_LOGIC_S16 = 6,/* the same 4 channels as int16 (4-channel 16-bit WAV), read as s / 32768.f              */
+   NFCB200_SIG_LOGIC_U8 = 7  /* 8-bit unsigned logic samples, the reference's logic WAVs (SignalStorageTask.cpp:485),
+                                read as b / 255.f (RecordDevice.cpp:244-245); only the _ch ISO 7816 calls take them     */
 } nfcb200_sigtype;
 
 enum { NFCB200_TECH_A = 0, NFCB200_TECH_B = 1, NFCB200_TECH_F = 2, NFCB200_TECH_V = 3 };
@@ -263,6 +265,22 @@ int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *samples, int sam
  */
 int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *samples, int sigtype, uint64_t n, uint32_t sample_rate, nfcb200_frame *out,
                                 uint64_t cap, uint64_t *n_out);
+
+/*
+ * The two calls above for logic captures of `channels` channels (4-8), laid out [n_streams][n_samples][channels] and
+ * [n][channels], in any logic format: NFCB200_SIG_LOGIC_F32, NFCB200_SIG_LOGIC_S16 or NFCB200_SIG_LOGIC_U8.  The reference
+ * reads a buffer's stride() channels per sample and decodes channels 0-3 (IO, CLK, RST, VCC: IsoTech.cpp:37-58,
+ * Iso7816.cpp:39-42); channels 4 and up are read past and never affect a frame.  channels outside 4-8 returns
+ * NFCB200_ERR_INVALID: with fewer than 4 the reference reads channels the sample does not have, with more than 8 it
+ * writes past its 8-channel sample (IsoTech.h:230-236).  Device samples of the batch call must be aligned to one channel
+ * (4 / 2 / 1 bytes); stream pitch and base need no other alignment.  A stream keeps its state, the last sample's channels
+ * 0-3 included, across pushes of different formats and channel counts.  Every other convention is that of
+ * nfcb200_iso7816_decode_batch and nfcb200_iso7816_stream_push, which mean channels = 4 and take float32 and int16 only.
+ */
+int nfcb200_iso7816_decode_batch_ch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t channels, uint32_t n_streams,
+                                    uint64_t n_samples, uint32_t sample_rate, nfcb200_frame *out, uint64_t cap, uint64_t *n_out);
+int nfcb200_iso7816_stream_push_ch(nfcb200_handle *h, const void *samples, int sigtype, uint32_t channels, uint64_t n, uint32_t sample_rate,
+                                   nfcb200_frame *out, uint64_t cap, uint64_t *n_out);
 
 /* frames of the ISO stream that did not fit an earlier push's buffer: up to cap of them, *n_left = how many remain */
 int nfcb200_iso7816_stream_pending(nfcb200_handle *h, nfcb200_frame *out, uint64_t cap, uint64_t *n_out, uint64_t *n_left);

@@ -12,13 +12,15 @@ from .binding import (  # noqa: F401
     SIG_IQ_S16,
     SIG_LOGIC_F32,
     SIG_LOGIC_S16,
+    SIG_LOGIC_U8,
     SIG_MAG_F32,
     SIG_MAG_S16,
     library_path,
     load_library,
     spectrum_shape,
 )
+from .logic_wav import LogicWav, read_logic_wav, write_logic_wav  # noqa: F401
 
 __all__ = ["Frame", "NfcB200Error", "NfcDecoder", "SIG_IQ_F32", "SIG_MAG_F32", "SIG_MAG_S16", "SIG_IQ_S16", "SIG_LOGIC_F32", "SIG_LOGIC_S16",
-           "library_path",
+           "SIG_LOGIC_U8", "LogicWav", "read_logic_wav", "write_logic_wav", "library_path",
            "load_library", "spectrum_shape"]

@@ -16,6 +16,7 @@ SIG_MAG_S16 = 3
 SIG_IQ_S16 = 4
 SIG_LOGIC_F32 = 5
 SIG_LOGIC_S16 = 6
+SIG_LOGIC_U8 = 7
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -130,6 +131,10 @@ def load_library():
                                                  C.POINTER(CFrame), C.c_uint64, C.POINTER(C.c_uint64)]
     lib.nfcb200_iso7816_stream_push.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.POINTER(CFrame), C.c_uint64,
                                                 C.POINTER(C.c_uint64)]
+    lib.nfcb200_iso7816_decode_batch_ch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32,
+                                                    C.POINTER(CFrame), C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.nfcb200_iso7816_stream_push_ch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint32, C.c_uint64, C.c_uint32, C.POINTER(CFrame),
+                                                   C.c_uint64, C.POINTER(C.c_uint64)]
     lib.nfcb200_iso7816_stream_pending.argtypes = [C.c_void_p, C.POINTER(CFrame), C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     lib.nfcb200_iso7816_stream_reset.argtypes = [C.c_void_p]
     lib.nfcb200_spectrum_shape.argtypes = [C.c_uint64, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
@@ -153,7 +158,18 @@ def spectrum_shape(n_samples, sample_rate, hop=None):
 
 
 _SIG_DTYPE = {SIG_IQ_F32: (np.float32, 2), SIG_MAG_F32: (np.float32, 1), SIG_MAG_S16: (np.int16, 1), SIG_IQ_S16: (np.int16, 2),
-              SIG_LOGIC_F32: (np.float32, 4), SIG_LOGIC_S16: (np.int16, 4)}
+              SIG_LOGIC_F32: (np.float32, 4), SIG_LOGIC_S16: (np.int16, 4), SIG_LOGIC_U8: (np.uint8, 4)}
+LOGIC_CHANNELS = range(4, 9)  # channels per logic sample the ISO 7816 calls take (include/nfcb200.h)
+
+
+def _logic_dtype(samples, sigtype):
+    """refuse 8-bit samples with another logic format, and anything but uint8 with SIG_LOGIC_U8: a conversion would read
+    the bytes b as b, not as b / 255.f"""
+    if _SIG_DTYPE.get(sigtype, (None, 0))[1] != 4:
+        raise NfcB200Error(-2, "signal type %d is not a logic format" % sigtype)
+    dt = str(getattr(samples, "dtype", ""))
+    if (sigtype == SIG_LOGIC_U8) != dt.endswith("uint8"):
+        raise NfcB200Error(-2, "signal type %d takes %s samples, got %s" % (sigtype, np.dtype(_SIG_DTYPE[sigtype][0]).name, dt or type(samples).__name__))
 
 
 class NfcDecoder:
@@ -285,7 +301,7 @@ class NfcDecoder:
         import torch
         if samples.is_cuda and samples.device.index != self._cfg.device:
             raise NfcB200Error(-2, "tensor on %s, decoder on cuda:%d" % (samples.device, self._cfg.device))
-        want = torch.float32 if dtype == np.float32 else torch.int16
+        want = {np.float32: torch.float32, np.int16: torch.int16, np.uint8: torch.uint8}[dtype]
         if samples.dtype != want:
             raise NfcB200Error(-2, "signal type %d takes %s samples, got a %s tensor" % (sigtype, want, samples.dtype))
         t = samples.contiguous()
@@ -374,33 +390,34 @@ class NfcDecoder:
         return int(nf.value)
 
     def iso7816_decode(self, samples, sigtype, sample_rate, cap=1 << 16, raw=False):
-        """ISO 7816 contact smart-card frames (lab::IsoDecoder) of 4-channel logic captures IO, CLK, RST, VCC: numpy
-        [n_streams, n_samples, 4] (or one stream [n_samples, 4]), float32 for SIG_LOGIC_F32 or int16 for SIG_LOGIC_S16, or a
-        torch tensor of the same shape (a CUDA tensor is decoded where it lies).  Frames are ordered by (stream, time).
-        raw=True returns (CFrame buffer, count) with every field, time_start / time_end / date_time included."""
-        if _SIG_DTYPE[sigtype][1] != 4:
-            raise NfcB200Error(-2, "signal type %d is not a 4-channel logic format" % sigtype)
+        """ISO 7816 contact smart-card frames (lab::IsoDecoder) of logic captures of C = 4-8 channels, IO, CLK, RST, VCC first:
+        numpy [n_streams, n_samples, C] (or one stream [n_samples, C]), float32 for SIG_LOGIC_F32, int16 for SIG_LOGIC_S16,
+        uint8 for SIG_LOGIC_U8 (read_logic_wav), or a torch tensor of the same shape (a CUDA tensor is decoded where it
+        lies).  Channels 4 and up are read past.  Frames are ordered by (stream, time).  raw=True returns (CFrame buffer,
+        count) with every field, time_start / time_end / date_time included."""
+        _logic_dtype(samples, sigtype)
         a, ptr, on_device = self._batch(samples, sigtype)
-        if len(a.shape) != 3 or a.shape[2] != 4:
-            raise NfcB200Error(-2, "logic samples must be [n_streams, n_samples, 4], got %s" % (tuple(a.shape),))
-        n_streams, n_samples = int(a.shape[0]), int(a.shape[1])
-        return self._with_room(lambda buf, cap, n: self._lib.nfcb200_iso7816_decode_batch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype,
-                                                                                       n_streams, n_samples, int(sample_rate), buf, cap, n), cap, raw)
+        if len(a.shape) != 3 or a.shape[2] not in LOGIC_CHANNELS:
+            raise NfcB200Error(-2, "logic samples must be [n_streams, n_samples, 4-8], got %s" % (tuple(a.shape),))
+        n_streams, n_samples, channels = int(a.shape[0]), int(a.shape[1]), int(a.shape[2])
+        return self._with_room(lambda buf, cap, n: self._lib.nfcb200_iso7816_decode_batch_ch(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype,
+                                                                                          channels, n_streams, n_samples, int(sample_rate), buf, cap, n),
+                               cap, raw)
 
     def iso7816_push(self, samples, sigtype, sample_rate, cap=4096, raw=False):
-        """lab::IsoDecoder::nextFrames(SignalBuffer) of one buffer of a live logic capture [n_samples, 4] (numpy, float32 for
-        SIG_LOGIC_F32 or int16 for SIG_LOGIC_S16): the frames it completes, every pending one included.  The decoder carries
-        over to the next push; a push at another sample rate restarts it.  Frames as iso7816_decode returns them; raw=True
-        gives a list of CFrame with every field."""
-        if _SIG_DTYPE.get(sigtype, (None, 0))[1] != 4:
-            raise NfcB200Error(-2, "signal type %d is not a 4-channel logic format" % sigtype)
+        """lab::IsoDecoder::nextFrames(SignalBuffer) of one buffer of a live logic capture [n_samples, C], C = 4-8 channels
+        (numpy, float32 for SIG_LOGIC_F32, int16 for SIG_LOGIC_S16, uint8 for SIG_LOGIC_U8): the frames it completes,
+        every pending one included.  The decoder carries over to the next push, whatever its format and channel count; a
+        push at another sample rate restarts it.  Frames as iso7816_decode returns them; raw=True gives a list of CFrame
+        with every field."""
+        _logic_dtype(samples, sigtype)
         a = np.ascontiguousarray(samples, dtype=_SIG_DTYPE[sigtype][0])
-        if a.ndim != 2 or a.shape[1] != 4:
-            raise NfcB200Error(-2, "logic samples must be [n_samples, 4], got %s" % (a.shape,))
+        if a.ndim != 2 or a.shape[1] not in LOGIC_CHANNELS:
+            raise NfcB200Error(-2, "logic samples must be [n_samples, 4-8], got %s" % (a.shape,))
         if a.shape[0] == 0:
             return self.iso7816_flush(cap, raw)
-        return self._iso_stream(lambda buf, cap, n: self._lib.nfcb200_iso7816_stream_push(self._h, a.ctypes.data, sigtype, a.shape[0], int(sample_rate),
-                                                                                          buf, cap, n), cap, raw)
+        return self._iso_stream(lambda buf, cap, n: self._lib.nfcb200_iso7816_stream_push_ch(self._h, a.ctypes.data, sigtype, a.shape[1], a.shape[0],
+                                                                                             int(sample_rate), buf, cap, n), cap, raw)
 
     def iso7816_flush(self, cap=4096, raw=False):
         """nextFrames({}) on the ISO stream: it decodes nothing (IsoTech.cpp:31-32); frames still pending are returned"""

@@ -1,7 +1,7 @@
 /*
- * iso7816.cu -- ISO 7816 contact smart-card traffic from 4-channel logic captures (lab::IsoDecoder, iso_decode.cuh):
- * nfcb200_iso7816_decode_batch for whole captures, nfcb200_iso7816_stream_* for one capture pushed buffer by buffer.  Both
- * run the same dense pass and the same walk.
+ * iso7816.cu -- ISO 7816 contact smart-card traffic from logic captures of 4-8 channels (lab::IsoDecoder, iso_decode.cuh):
+ * nfcb200_iso7816_decode_batch(_ch) for whole captures, nfcb200_iso7816_stream_* for one capture pushed buffer by buffer.
+ * All run the same dense pass and the same walk.
  */
 #include <numeric>
 
@@ -10,10 +10,40 @@
 
 using namespace nfcb200;
 
+// bytes of one channel of a logic sample
+static uint32_t iso_elem_bytes(int sigtype)
+{
+   return sigtype == NFCB200_SIG_LOGIC_F32 ? 4 : sigtype == NFCB200_SIG_LOGIC_S16 ? 2 : 1;
+}
+
+// one dense pass over sc streams of `channels` channels at dSamples: float32 / int16 at stride 4 aligned to the sample and
+// 8-bit at stride 4 aligned to 16 bytes load samples directly, everything else is staged in shared memory (iso_decode.cuh)
+static void launch_edges(cudaStream_t st, int sigtype, uint32_t channels, uint32_t sc, const IsoEdgesArgs &E)
+{
+   const dim3 grid(E.n_tiles, sc);
+   const uintptr_t at = (uintptr_t) E.samples;
+   const uint32_t bps = channels * iso_elem_bytes(sigtype);
+   if (channels == 4 && sigtype != NFCB200_SIG_LOGIC_U8 && at % bps == 0)
+   {
+      if (sigtype == NFCB200_SIG_LOGIC_S16)
+         iso_edges_kernel<true><<<grid, ISO_THREADS, 0, st>>>(E);
+      else
+         iso_edges_kernel<false><<<grid, ISO_THREADS, 0, st>>>(E);
+   }
+   else if (channels == 4 && at % 16 == 0 && (sc == 1 || E.n_samples % 4 == 0))
+      iso_edges_u8x4_kernel<<<grid, ISO_THREADS, 0, st>>>(E);
+   else if (sigtype == NFCB200_SIG_LOGIC_F32)
+      iso_edges_staged_kernel<float><<<grid, ISO_THREADS, iso_stage_bytes<float>(bps), st>>>(E, channels);
+   else if (sigtype == NFCB200_SIG_LOGIC_S16)
+      iso_edges_staged_kernel<int16_t><<<grid, ISO_THREADS, iso_stage_bytes<int16_t>(bps), st>>>(E, channels);
+   else
+      iso_edges_staged_kernel<uint8_t><<<grid, ISO_THREADS, iso_stage_bytes<uint8_t>(bps), st>>>(E, channels);
+}
+
 // the dense pass over sc streams at dSamples, again with room for a line event and a CLK falling edge at every sample
 // when a tile overflows the first try's slots; E holds the slots the walk reads
-static int edge_pass(cudaStream_t st, bool s16, const void *dSamples, uint32_t sc, uint64_t n_samples, float4 last, nfcb200_handle::IsoEvents &B,
-                     uint32_t *overflow, IsoEdgesArgs &E)
+static int edge_pass(cudaStream_t st, int sigtype, uint32_t channels, const void *dSamples, uint32_t sc, uint64_t n_samples, float4 last,
+                     nfcb200_handle::IsoEvents &B, uint32_t *overflow, IsoEdgesArgs &E)
 {
    const uint32_t nTiles = (uint32_t) ((n_samples + ISO_TILE - 1) / ISO_TILE);
    int rc;
@@ -34,11 +64,7 @@ static int edge_pass(cudaStream_t st, bool s16, const void *dSamples, uint32_t s
       E.line = B.line.as<uint32_t>();
       E.clk = B.clk.as<uint16_t>();
       CUDA_TRY(cudaMemsetAsync(E.overflow, 0, 4, st));
-      const dim3 grid(nTiles, sc);
-      if (s16)
-         iso_edges_kernel<true><<<grid, ISO_THREADS, 0, st>>>(E);
-      else
-         iso_edges_kernel<false><<<grid, ISO_THREADS, 0, st>>>(E);
+      launch_edges(st, sigtype, channels, sc, E);
       CUDA_TRY(cudaGetLastError());
       uint32_t over = 0;
       CUDA_TRY(cudaMemcpyAsync(&over, E.overflow, 4, cudaMemcpyDeviceToHost, st));
@@ -81,15 +107,24 @@ static int walk_pass(cudaStream_t st, const IsoEdgesArgs &E, IsoWalkArgs &W, uin
    }
 }
 
-extern "C" int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams,
-                                            uint64_t n_samples, uint32_t sample_rate, nfcb200_frame *out, uint64_t cap, uint64_t *n_out)
+static bool is_logic(int sigtype)
 {
-   if (!h)
-      return fail(NFCB200_ERR_INVALID, "null handle");
-   if (n_out)
-      *n_out = 0;
-   if (sigtype != NFCB200_SIG_LOGIC_F32 && sigtype != NFCB200_SIG_LOGIC_S16)
-      return fail(NFCB200_ERR_INVALID, "signal type %d is not a 4-channel logic format", sigtype);
+   return sigtype == NFCB200_SIG_LOGIC_F32 || sigtype == NFCB200_SIG_LOGIC_S16 || sigtype == NFCB200_SIG_LOGIC_U8;
+}
+
+// channels outside 4-8: below 4 the reference reads channels the buffer does not have, above 8 it writes past its 8-channel
+// sample (IsoTech.cpp:37-58)
+static int check_channels(uint32_t channels)
+{
+   if (channels < 4 || channels > 8)
+      return fail(NFCB200_ERR_INVALID, "%u channels: logic samples have 4 to 8", channels);
+   return 0;
+}
+
+// the batch decode of both entry points; `align`: the alignment device samples must have
+static int iso_batch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t channels, uint32_t align, uint32_t n_streams,
+                     uint64_t n_samples, uint32_t sample_rate, nfcb200_frame *out, uint64_t cap, uint64_t *n_out)
+{
    if (sample_rate == 0)
       return fail(NFCB200_ERR_INVALID, "sample rate of 0");
    if (!samples || n_streams == 0 || n_samples == 0)
@@ -98,10 +133,9 @@ extern "C" int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *sampl
       return fail(NFCB200_ERR_INVALID, "null frame buffer");
    if (n_samples >= 0xFFFFFFFFull)
       return fail(NFCB200_ERR_UNSUPPORTED, "streams of 2^32 - 1 samples or more exceed the 32-bit sample clock of the reference (IsoTech.h:221)");
-   const bool s16 = sigtype == NFCB200_SIG_LOGIC_S16;
-   const uint64_t bs = s16 ? 8 : 16;
-   if (samples_on_device && ((uintptr_t) samples % bs))
-      return fail(NFCB200_ERR_INVALID, "device samples not aligned to %u bytes", (unsigned) bs);
+   const uint64_t bs = (uint64_t) channels * iso_elem_bytes(sigtype);
+   if (samples_on_device && ((uintptr_t) samples % align))
+      return fail(NFCB200_ERR_INVALID, "device samples not aligned to %u bytes", align);
 
    CUDA_TRY(cudaSetDevice(h->device));
    cudaStream_t st = h->stream;
@@ -117,7 +151,7 @@ extern "C" int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *sampl
       if ((rc = I.streamCount.reserve((uint64_t) sc * 4)) || (rc = I.first.reserve((uint64_t) sc * 8)))
          return rc;
       IsoEdgesArgs E;
-      if ((rc = edge_pass(st, s16, dSamples, sc, n_samples, make_float4(0, 0, 0, 0), I.ev, I.ctr.as<uint32_t>() + 1, E)))
+      if ((rc = edge_pass(st, sigtype, channels, dSamples, sc, n_samples, make_float4(0, 0, 0, 0), I.ev, I.ctr.as<uint32_t>() + 1, E)))
          return rc;
       IsoWalkArgs W = {};
       W.stream0 = s0;
@@ -158,6 +192,34 @@ extern "C" int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *sampl
    return 0;
 }
 
+extern "C" int nfcb200_iso7816_decode_batch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams,
+                                            uint64_t n_samples, uint32_t sample_rate, nfcb200_frame *out, uint64_t cap, uint64_t *n_out)
+{
+   if (!h)
+      return fail(NFCB200_ERR_INVALID, "null handle");
+   if (n_out)
+      *n_out = 0;
+   if (sigtype != NFCB200_SIG_LOGIC_F32 && sigtype != NFCB200_SIG_LOGIC_S16)
+      return fail(NFCB200_ERR_INVALID, "signal type %d is not a 4-channel logic format", sigtype);
+   return iso_batch(h, samples, samples_on_device, sigtype, 4, sigtype == NFCB200_SIG_LOGIC_S16 ? 8 : 16, n_streams, n_samples, sample_rate, out, cap,
+                    n_out);
+}
+
+extern "C" int nfcb200_iso7816_decode_batch_ch(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t channels,
+                                               uint32_t n_streams, uint64_t n_samples, uint32_t sample_rate, nfcb200_frame *out, uint64_t cap,
+                                               uint64_t *n_out)
+{
+   if (!h)
+      return fail(NFCB200_ERR_INVALID, "null handle");
+   if (n_out)
+      *n_out = 0;
+   if (!is_logic(sigtype))
+      return fail(NFCB200_ERR_INVALID, "signal type %d is not a logic format", sigtype);
+   if (int rc = check_channels(channels))
+      return rc;
+   return iso_batch(h, samples, samples_on_device, sigtype, channels, iso_elem_bytes(sigtype), n_streams, n_samples, sample_rate, out, cap, n_out);
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // streaming: one capture, buffer by buffer
 // ---------------------------------------------------------------------------------------------------------------------
@@ -189,13 +251,10 @@ extern "C" int nfcb200_iso7816_stream_pending(nfcb200_handle *h, nfcb200_frame *
    return 0;
 }
 
-extern "C" int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *samples, int sigtype, uint64_t n, uint32_t sample_rate, nfcb200_frame *out,
-                                           uint64_t cap, uint64_t *n_out)
+// the push of both entry points (sigtype and channels checked)
+static int iso_push(nfcb200_handle *h, const void *samples, int sigtype, uint32_t channels, uint64_t n, uint32_t sample_rate, nfcb200_frame *out,
+                    uint64_t cap, uint64_t *n_out)
 {
-   if (!h)
-      return fail(NFCB200_ERR_INVALID, "null handle");
-   if (n_out)
-      *n_out = 0;
    if (cap && !out)
       return fail(NFCB200_ERR_INVALID, "null frame buffer");
    auto &S = h->isoStream;
@@ -204,8 +263,6 @@ extern "C" int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *sample
    // the next buffer picks its loop afresh anyway; only frames still pending are delivered
    if (n)
    {
-      if (sigtype != NFCB200_SIG_LOGIC_F32 && sigtype != NFCB200_SIG_LOGIC_S16)
-         return fail(NFCB200_ERR_INVALID, "signal type %d is not a 4-channel logic format", sigtype);
       if (!samples)
          return fail(NFCB200_ERR_INVALID, "null samples");
       if (sample_rate == 0)
@@ -216,8 +273,7 @@ extern "C" int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *sample
       if (base + n >= 0xFFFFFFFFull)
          return fail(NFCB200_ERR_UNSUPPORTED, "stream position would pass 2^32 - 1 samples, the 32-bit sample clock of the reference (IsoTech.h:221): "
                                               "call nfcb200_iso7816_stream_reset");
-      const bool s16 = sigtype == NFCB200_SIG_LOGIC_S16;
-      const uint64_t bs = s16 ? 8 : 16;
+      const uint64_t bs = (uint64_t) channels * iso_elem_bytes(sigtype);
 
       CUDA_TRY(cudaSetDevice(h->device));
       cudaStream_t st = h->stream;
@@ -232,7 +288,7 @@ extern "C" int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *sample
          CUDA_TRY(cudaMemsetAsync(state + S.cur, 0, sizeof(iso7816::IsoStreamState), st));
 
       IsoEdgesArgs E;
-      if ((rc = edge_pass(st, s16, S.in.ptr, 1, n, make_float4(S.last[0], S.last[1], S.last[2], S.last[3]), S.ev, S.ctr.as<uint32_t>() + 1, E)))
+      if ((rc = edge_pass(st, sigtype, channels, S.in.ptr, 1, n, make_float4(S.last[0], S.last[1], S.last[2], S.last[3]), S.ev, S.ctr.as<uint32_t>() + 1, E)))
          return rc;
       IsoWalkArgs W = {};
       W.sample_rate = sample_rate;
@@ -261,9 +317,12 @@ extern "C" int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *sample
       S.init = true;
       S.rate = sample_rate;
       S.clock = (uint32_t) (base + n);
+      // channels 0-3 of the last sample, as the decoder read them
       const unsigned char *tail = (const unsigned char *) samples + (n - 1) * bs;
       for (int c = 0; c < 4; c++)
-         S.last[c] = s16 ? ((const int16_t *) tail)[c] / 32768.f : ((const float *) tail)[c];
+         S.last[c] = sigtype == NFCB200_SIG_LOGIC_S16 ? ((const int16_t *) tail)[c] / 32768.f
+                     : sigtype == NFCB200_SIG_LOGIC_U8 ? tail[c] / 255.f
+                                                       : ((const float *) tail)[c];
    }
 
    const uint64_t nf = S.pending.size();
@@ -275,4 +334,31 @@ extern "C" int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *sample
       return fail(NFCB200_ERR_CAPACITY, "%llu frames decoded but room for %llu only: the rest waits in nfcb200_iso7816_stream_pending",
                   (unsigned long long) nf, (unsigned long long) cap);
    return 0;
+}
+
+extern "C" int nfcb200_iso7816_stream_push(nfcb200_handle *h, const void *samples, int sigtype, uint64_t n, uint32_t sample_rate, nfcb200_frame *out,
+                                           uint64_t cap, uint64_t *n_out)
+{
+   if (!h)
+      return fail(NFCB200_ERR_INVALID, "null handle");
+   if (n_out)
+      *n_out = 0;
+   if (n && sigtype != NFCB200_SIG_LOGIC_F32 && sigtype != NFCB200_SIG_LOGIC_S16)
+      return fail(NFCB200_ERR_INVALID, "signal type %d is not a 4-channel logic format", sigtype);
+   return iso_push(h, samples, sigtype, 4, n, sample_rate, out, cap, n_out);
+}
+
+extern "C" int nfcb200_iso7816_stream_push_ch(nfcb200_handle *h, const void *samples, int sigtype, uint32_t channels, uint64_t n, uint32_t sample_rate,
+                                              nfcb200_frame *out, uint64_t cap, uint64_t *n_out)
+{
+   if (!h)
+      return fail(NFCB200_ERR_INVALID, "null handle");
+   if (n_out)
+      *n_out = 0;
+   if (n && !is_logic(sigtype))
+      return fail(NFCB200_ERR_INVALID, "signal type %d is not a logic format", sigtype);
+   if (n)
+      if (int rc = check_channels(channels))
+         return rc;
+   return iso_push(h, samples, sigtype, channels, n, sample_rate, out, cap, n_out);
 }

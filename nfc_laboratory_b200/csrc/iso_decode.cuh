@@ -9,6 +9,9 @@
  *                          written, and the call runs the pass again with room for one of each at every sample: a
  *                          two-level clock has at most ISO_TILE / 2 falling edges per tile, but a clock with more levels
  *                          (noise, a staircase, a ramp) can fall on every sample.
+ *   iso_edges_u8x4_kernel  the same pass over 8-bit samples at stride 4 (one 32-bit word per sample, 16-byte loads).
+ *   iso_edges_staged_kernel<T>  the same pass at any stride 4-8 and alignment: each sub-tile of iso_sub<T>() samples is copied
+ *                          to shared memory with 16-byte loads, then channels 0-3 are picked there.
  *   iso_walk_kernel        one warp per stream runs iso_walk() over the tiles' events in order (the lanes evaluate 32
  *                          clock measurements at a time) and appends its frames to a pool with the stream index and the
  *                          frame's rank in its stream, and the stream's frame count.  A stream pushed buffer by buffer
@@ -68,6 +71,134 @@ __device__ __forceinline__ void iso_load(const void *base, uint64_t i, float d[4
    }
 }
 
+// A tile's flags as its threads hold them: fl[j * K + k] is sample j * ISO_THREADS * K + threadIdx.x * K + k of the tile, so
+// the samples run in (j, warp, lane, k) order.  iso_tile_count() is called once per j as the flags come, iso_tile_scan()
+// once, iso_tile_write() then puts every event in its slot in sample order.
+template <uint32_t K>
+struct IsoTileSlots
+{
+   static constexpr uint32_t J = ISO_PER_THREAD / K, W = ISO_THREADS / 32;
+   uint32_t warpLine[J][W], warpClk[J][W]; // events of each (j, warp)
+   uint32_t offLine[J][W], offClk[J][W];   // their first slot
+   uint32_t total[2];
+};
+
+template <uint32_t K>
+__device__ __forceinline__ void iso_tile_count(IsoTileSlots<K> &sh, const uint32_t *fl, uint32_t j)
+{
+   using namespace iso7816;
+   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+   uint32_t nl = 0, nc = 0;
+#pragma unroll
+   for (uint32_t k = 0; k < K; k++)
+   {
+      nl += __popc(__ballot_sync(~0u, (fl[j * K + k] & F_LINE) != 0));
+      nc += __popc(__ballot_sync(~0u, (fl[j * K + k] & F_CLK_FALL) != 0));
+   }
+   if (lane == 0)
+   {
+      sh.warpLine[j][warp] = nl;
+      sh.warpClk[j][warp] = nc;
+   }
+}
+
+// exclusive scan of the per-(j, warp) counts in sample order, by warp 0 (between two barriers)
+template <uint32_t K>
+__device__ __forceinline__ void iso_tile_scan(IsoTileSlots<K> &sh)
+{
+   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+   if (warp == 0)
+   {
+      constexpr uint32_t N = IsoTileSlots<K>::J * IsoTileSlots<K>::W, PER = N / 32;
+      uint32_t *wl = &sh.warpLine[0][0], *wc = &sh.warpClk[0][0];
+      uint32_t sl = 0, sc = 0;
+      for (uint32_t k = 0; k < PER; k++)
+      {
+         sl += wl[lane * PER + k];
+         sc += wc[lane * PER + k];
+      }
+      uint32_t il = sl, ic = sc;
+      for (uint32_t o = 1; o < 32; o <<= 1)
+      {
+         const uint32_t vl = __shfl_up_sync(~0u, il, o), vc = __shfl_up_sync(~0u, ic, o);
+         if (lane >= o)
+         {
+            il += vl;
+            ic += vc;
+         }
+      }
+      uint32_t el = il - sl, ec = ic - sc;
+      for (uint32_t k = 0; k < PER; k++)
+      {
+         const uint32_t cl = wl[lane * PER + k], cc = wc[lane * PER + k];
+         (&sh.offLine[0][0])[lane * PER + k] = el;
+         (&sh.offClk[0][0])[lane * PER + k] = ec;
+         el += cl;
+         ec += cc;
+      }
+      if (lane == 31)
+      {
+         sh.total[0] = il;
+         sh.total[1] = ic;
+      }
+   }
+}
+
+template <uint32_t K>
+__device__ __forceinline__ void iso_tile_write(const IsoEdgesArgs &a, const IsoTileSlots<K> &sh, const uint32_t *fl)
+{
+   using namespace iso7816;
+   const uint32_t tile = blockIdx.x, stream = blockIdx.y;
+   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+   const uint64_t slot = (uint64_t) stream * a.n_tiles + tile;
+   uint32_t *line = a.line + slot * a.line_cap;
+   uint16_t *clk = a.clk + slot * a.clk_cap;
+   const uint32_t below = (1u << lane) - 1;
+#pragma unroll
+   for (uint32_t j = 0; j < IsoTileSlots<K>::J; j++)
+   {
+      uint32_t bl[K], bc[K], kl = sh.offLine[j][warp], kc = sh.offClk[j][warp];
+#pragma unroll
+      for (uint32_t k = 0; k < K; k++)
+      {
+         bl[k] = __ballot_sync(~0u, (fl[j * K + k] & F_LINE) != 0);
+         bc[k] = __ballot_sync(~0u, (fl[j * K + k] & F_CLK_FALL) != 0);
+      }
+#pragma unroll
+      for (uint32_t k = 0; k < K; k++) // the events of the lanes below, then this lane's own earlier samples
+      {
+         kl += __popc(bl[k] & below);
+         kc += __popc(bc[k] & below);
+      }
+#pragma unroll
+      for (uint32_t k = 0; k < K; k++)
+      {
+         const uint32_t f = fl[j * K + k], off = (j * ISO_THREADS + threadIdx.x) * K + k;
+         if (f & F_LINE)
+         {
+            if (kl < a.line_cap)
+               line[kl] = off | (f & ~F_CLK_FALL) << 12;
+            kl++;
+         }
+         if (f & F_CLK_FALL)
+         {
+            if (kc < a.clk_cap)
+               clk[kc] = (uint16_t) off;
+            kc++;
+         }
+      }
+   }
+   if (threadIdx.x == 0)
+   {
+      a.line_count[slot] = sh.total[0];
+      a.clk_count[slot] = sh.total[1];
+      if (sh.total[0] > a.line_cap || sh.total[1] > a.clk_cap)
+         atomicOr(a.overflow, 1u);
+   }
+}
+
+// float32 / int16 at stride 4, the stream aligned to the sample (16 / 8 bytes): one vector load per sample.  It keeps its
+// own copy of the tile's count, scan and write (those of IsoTileSlots with K = 1), so its code stays as it was measured.
 template <bool S16>
 __global__ void __launch_bounds__(ISO_THREADS) iso_edges_kernel(const IsoEdgesArgs a)
 {
@@ -170,6 +301,218 @@ __global__ void __launch_bounds__(ISO_THREADS) iso_edges_kernel(const IsoEdgesAr
       if (total[0] > a.line_cap || total[1] > a.clk_cap)
          atomicOr(a.overflow, 1u);
    }
+}
+
+// flags of an 8-bit sample (4 channels in the low bytes of w) after the one in p, compared as integers (sample_flags)
+__device__ __forceinline__ uint32_t iso_u8_flags(uint32_t w, uint32_t p)
+{
+   const int d[4] = {(int) (w & 0xFF), (int) (w >> 8 & 0xFF), (int) (w >> 16 & 0xFF), (int) (w >> 24)};
+   const int l[4] = {(int) (p & 0xFF), (int) (p >> 8 & 0xFF), (int) (p >> 16 & 0xFF), (int) (p >> 24)};
+   return iso7816::sample_flags(d, l);
+}
+
+// the first sample of a stream after a.last, in float as RecordDevice reads 8-bit samples (b / 255.f): a pushed stream's
+// previous sample can come from a buffer of another format
+__device__ __forceinline__ uint32_t iso_u8_first_flags(uint32_t w, const float4 &last)
+{
+   const float d[4] = {(w & 0xFF) / 255.f, (w >> 8 & 0xFF) / 255.f, (w >> 16 & 0xFF) / 255.f, (w >> 24) / 255.f};
+   const float l[4] = {last.x, last.y, last.z, last.w};
+   return iso7816::sample_flags(d, l);
+}
+
+// 8-bit samples at stride 4, the streams' base and pitch 16-byte aligned: a sample is one 32-bit word, a thread loads 4
+// consecutive samples with one 16-byte load and takes the sample before them from the lane below (lane 0: one word load)
+__global__ void __launch_bounds__(ISO_THREADS) iso_edges_u8x4_kernel(const IsoEdgesArgs a)
+{
+   constexpr uint32_t K = 4;
+   __shared__ IsoTileSlots<K> sh;
+
+   const uint32_t tile = blockIdx.x, stream = blockIdx.y, lane = threadIdx.x & 31;
+   const uint64_t t0 = (uint64_t) tile * ISO_TILE, n = a.n_samples;
+   const uint32_t *base = (const uint32_t *) a.samples + (uint64_t) stream * n;
+
+   // every load first, so that a thread has all of them in flight at once
+   constexpr uint32_t J = IsoTileSlots<K>::J;
+   uint32_t w[ISO_PER_THREAD], p[J];
+#pragma unroll
+   for (uint32_t j = 0; j < J; j++)
+   {
+      const uint64_t i = t0 + (j * ISO_THREADS + threadIdx.x) * K;
+      if (i + K <= n)
+      {
+         const uint4 v = __ldg((const uint4 *) (base + i));
+         w[j * K] = v.x;
+         w[j * K + 1] = v.y;
+         w[j * K + 2] = v.z;
+         w[j * K + 3] = v.w;
+      }
+      else
+      {
+#pragma unroll
+         for (uint32_t k = 0; k < K; k++)
+            w[j * K + k] = i + k < n ? __ldg(base + i + k) : 0u;
+      }
+      p[j] = lane == 0 && i > 0 && i < n ? __ldg(base + i - 1) : 0u;
+   }
+
+   uint32_t fl[ISO_PER_THREAD];
+#pragma unroll
+   for (uint32_t j = 0; j < J; j++)
+   {
+      const uint64_t i = t0 + (j * ISO_THREADS + threadIdx.x) * K;
+      const uint32_t up = __shfl_up_sync(~0u, w[j * K + K - 1], 1);
+      if (lane)
+         p[j] = up;
+#pragma unroll
+      for (uint32_t k = 0; k < K; k++)
+      {
+         const uint64_t s = i + k;
+         fl[j * K + k] = s >= n ? 0u : s == 0 ? iso_u8_first_flags(w[0], a.last) : iso_u8_flags(w[j * K + k], k ? w[j * K + k - 1] : p[j]);
+      }
+      iso_tile_count<K>(sh, fl, j);
+   }
+   __syncthreads();
+   iso_tile_scan<K>(sh);
+   __syncthreads();
+   iso_tile_write<K>(a, sh, fl);
+}
+
+// channels 0-3 of sample `at` of a staged sub-tile, as the decoder reads them: float32 as is, int16 as s / 32768.f; 8-bit
+// samples as their integer values (their flags are those of b / 255.f, sample_flags)
+template <class T>
+struct IsoStaged;
+
+template <>
+struct IsoStaged<float>
+{
+   using V = float;
+   static __device__ __forceinline__ void load(const unsigned char *p, V d[4])
+   {
+      for (int c = 0; c < 4; c++)
+         d[c] = ((const float *) p)[c];
+   }
+   static __device__ __forceinline__ void last(const float4 &l, V d[4])
+   {
+      d[0] = l.x, d[1] = l.y, d[2] = l.z, d[3] = l.w;
+   }
+};
+
+template <>
+struct IsoStaged<int16_t>
+{
+   using V = float;
+   static __device__ __forceinline__ void load(const unsigned char *p, V d[4])
+   {
+      for (int c = 0; c < 4; c++)
+         d[c] = ((const int16_t *) p)[c] / 32768.f;
+   }
+   static __device__ __forceinline__ void last(const float4 &l, V d[4])
+   {
+      IsoStaged<float>::last(l, d);
+   }
+};
+
+template <>
+struct IsoStaged<uint8_t>
+{
+   using V = int;
+   static __device__ __forceinline__ void load(const unsigned char *p, V d[4])
+   {
+      for (int c = 0; c < 4; c++)
+         d[c] = p[c];
+   }
+};
+
+// samples a staged kernel reads into shared memory at a time: 32 KB at 8 channels (a whole tile of 8-bit samples, half a
+// tile of int16, a quarter of float32), so that 4 CTAs of 256 threads fit an SM by shared memory as by registers
+template <class T>
+__host__ __device__ constexpr uint32_t iso_sub()
+{
+   return 32768 / (8 * sizeof(T));
+}
+
+// bytes of shared memory a staged kernel needs at `bps` bytes per sample: a sub-tile and the sample before it, from the
+// 16-byte boundary below them to the one above
+template <class T>
+__host__ __device__ constexpr uint32_t iso_stage_bytes(uint32_t bps)
+{
+   return ((iso_sub<T>() + 1) * bps + 31) & ~15u;
+}
+
+// Any element type T at any stride 4-8, any alignment of the streams' base and pitch (T-aligned): the tile is read
+// iso_sub<T>() samples at a time.  The threads copy the sub-tile's bytes, and the sample before it, into shared memory with
+// coalesced 16-byte loads where the bytes are 16-byte aligned and byte loads for the up to 15 bytes at either end, then
+// each thread picks channels 0-3 of its samples there.  Channels 4 and up are read past.
+template <class T>
+__global__ void __launch_bounds__(ISO_THREADS) iso_edges_staged_kernel(const IsoEdgesArgs a, uint32_t channels)
+{
+   using V = typename IsoStaged<T>::V;
+   constexpr uint32_t SUB = iso_sub<T>();
+   __shared__ IsoTileSlots<1> sh;
+   extern __shared__ uint4 stage[];
+   unsigned char *sb = (unsigned char *) stage;
+
+   const uint32_t tile = blockIdx.x, stream = blockIdx.y;
+   const uint64_t t0 = (uint64_t) tile * ISO_TILE, n = a.n_samples;
+   const uint32_t bps = channels * (uint32_t) sizeof(T);
+   const unsigned char *base = (const unsigned char *) a.samples + (uint64_t) stream * n * bps;
+
+   uint32_t fl[ISO_PER_THREAD];
+#pragma unroll
+   for (uint32_t sub = 0; sub < ISO_TILE / SUB; sub++)
+   {
+      const uint64_t s0 = t0 + sub * SUB;
+      const uint64_t first = s0 ? s0 - 1 : 0, end = s0 + SUB < n ? s0 + SUB : n;
+      const uintptr_t lo = (uintptr_t) (base + first * bps), hi = (uintptr_t) (base + end * bps);
+      const uintptr_t a0 = lo & ~(uintptr_t) 15, w0 = (lo + 15) & ~(uintptr_t) 15, w1 = hi & ~(uintptr_t) 15;
+      __syncthreads(); // the previous sub-tile is read
+      if (s0 < n)
+      {
+         if (w0 <= w1)
+         {
+            for (uintptr_t k = threadIdx.x; k < (w1 - w0) / 16; k += ISO_THREADS)
+               stage[(w0 - a0) / 16 + k] = __ldg((const uint4 *) w0 + k);
+            if (threadIdx.x < w0 - lo)
+               sb[lo - a0 + threadIdx.x] = __ldg((const unsigned char *) lo + threadIdx.x);
+            if (threadIdx.x < hi - w1)
+               sb[w1 - a0 + threadIdx.x] = __ldg((const unsigned char *) w1 + threadIdx.x);
+         }
+         else if (threadIdx.x < hi - lo) // within one 16-byte word
+            sb[lo - a0 + threadIdx.x] = __ldg((const unsigned char *) lo + threadIdx.x);
+      }
+      __syncthreads();
+#pragma unroll
+      for (uint32_t jj = 0; jj < SUB / ISO_THREADS; jj++)
+      {
+         const uint32_t j = sub * (SUB / ISO_THREADS) + jj;
+         const uint64_t i = s0 + jj * ISO_THREADS + threadIdx.x;
+         uint32_t f = 0;
+         if (i < n)
+         {
+            const unsigned char *p = sb + (lo - a0) + (i - first) * bps;
+            V d[4], l[4];
+            IsoStaged<T>::load(p, d);
+            if (i > 0)
+            {
+               IsoStaged<T>::load(p - bps, l);
+               f = iso7816::sample_flags(d, l);
+            }
+            else if constexpr (sizeof(T) == 1)
+               f = iso_u8_first_flags(p[0] | p[1] << 8 | p[2] << 16 | (uint32_t) p[3] << 24, a.last);
+            else
+            {
+               IsoStaged<T>::last(a.last, l);
+               f = iso7816::sample_flags(d, l);
+            }
+         }
+         fl[j] = f;
+         iso_tile_count<1>(sh, fl, j);
+      }
+   }
+   __syncthreads();
+   iso_tile_scan<1>(sh);
+   __syncthreads();
+   iso_tile_write<1>(a, sh, fl);
 }
 
 // the event source of iso_walk(): the per-tile slots of one stream, read in tile order, at absolute samples from `base`

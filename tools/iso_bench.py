@@ -1,12 +1,15 @@
-"""Benchmark of the ISO 7816 decoder (nfcb200_iso7816_decode_batch) on one GPU.
+"""Benchmark of the ISO 7816 decoder (nfcb200_iso7816_decode_batch, nfcb200_iso7816_decode_batch_ch) on one GPU.
 
 Default batch: 128 streams of 2.5e7 LOGIC_F32 samples (1 s at 25 MS/s each, 51.2 GB), assembled on the device from a
 seeded synthetic session (nfc_laboratory_b200.synth.iso7816_capture, T=1, repeated back to back: every repetition is a
-full power-up, ATR, PPS and block exchange).  Reports, as one JSON line:
+full power-up, ATR, PPS and block exchange).  --sigtype f32 / s16 / u8 (or the number) picks the sample format,
+--channels 4-8 the stride (the channels past VCC are seeded noise); u8 samples are the capture clipped to [0, 1] as
+RecordDevice writes it.  Reports, as one JSON line:
   - the whole call's time and rate (host clock around a synchronised call, median of --reps after a warm-up), with the
     frames converted to Python tuples and without (raw ctypes records: the C entry point alone),
   - kernel times of the edge pass and the walk from torch.profiler, in a run of their own,
   - the edge pass's input bytes over its kernel time, as a share of the H100 SXM's 3.35 TB/s,
+  - with --pinned, the C entry point again from a pinned host copy of the batch (the input is copied in ~1 GB groups),
   - the card's name, power limit and SM clocks, read in the same run.
 Writes the profiler trace under --out when given."""
 import argparse
@@ -26,6 +29,11 @@ import nfc_laboratory_b200 as N  # noqa: E402
 from nfc_laboratory_b200 import synth as S  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
+SIGTYPES = {"f32": N.SIG_LOGIC_F32, "s16": N.SIG_LOGIC_S16, "u8": N.SIG_LOGIC_U8}
+
+
+def sigtype(v):
+    return SIGTYPES[v] if v in SIGTYPES else int(v)
 
 
 def card():
@@ -42,19 +50,26 @@ def main():
     ap.add_argument("--streams", type=int, default=128)
     ap.add_argument("--samples", type=int, default=25_000_000)
     ap.add_argument("--rate", type=int, default=25_000_000)
-    ap.add_argument("--sigtype", type=int, default=N.SIG_LOGIC_F32)
+    ap.add_argument("--sigtype", type=sigtype, default=N.SIG_LOGIC_F32)
+    ap.add_argument("--channels", type=int, default=4)
+    ap.add_argument("--pinned", action="store_true")
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
 
     dev = torch.device("cuda:0")
     one = S.iso7816_capture("t1_lrc", a.rate, seed=11)
+    if a.channels > 4:
+        extra = np.random.default_rng(a.channels).random((len(one), a.channels - 4), dtype=np.float32)
+        one = np.concatenate([one, extra], axis=1)
     if a.sigtype == N.SIG_LOGIC_S16:
         one = (one * 32767).astype(np.int16)
+    elif a.sigtype == N.SIG_LOGIC_U8:
+        one = N.logic_wav.logic_bytes(np.clip(one, 0, 1))
     base = torch.from_numpy(one).to(dev)
     reps = -(-a.samples // base.shape[0])
     stream = base.repeat(reps, 1)[:a.samples]
-    batch = torch.empty((a.streams, a.samples, 4), dtype=base.dtype, device=dev)
+    batch = torch.empty((a.streams, a.samples, a.channels), dtype=base.dtype, device=dev)
     for s in range(a.streams):
         batch[s].copy_(stream)
     del stream
@@ -82,6 +97,18 @@ def main():
         torch.cuda.synchronize()
         raw.append(time.perf_counter() - t0)
     entry = float(np.median(raw))
+    pinned = None
+    if a.pinned:
+        host = torch.empty(batch.shape, dtype=batch.dtype, pin_memory=True)
+        host.copy_(batch)
+        d.iso7816_decode(host, a.sigtype, a.rate, raw=True)
+        ph = []
+        for _ in range(a.reps):
+            t0 = time.perf_counter()
+            d.iso7816_decode(host, a.sigtype, a.rate, raw=True)
+            ph.append(time.perf_counter() - t0)
+        pinned = float(np.median(ph))
+        del host
 
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -94,7 +121,7 @@ def main():
     for e in prof.events():
         name = e.name
         dt = e.device_time_total
-        if "iso_edges_kernel" in name:
+        if "iso_edges" in name:
             kt["edges"] += dt / 1e3
         elif "iso_walk_kernel" in name:
             kt["walk"] += dt / 1e3
@@ -102,11 +129,13 @@ def main():
 
     res = {
         "card": card(),
-        "streams": a.streams, "samples_per_stream": a.samples, "sigtype": a.sigtype, "input_bytes": in_bytes,
+        "streams": a.streams, "samples_per_stream": a.samples, "sigtype": a.sigtype, "channels": a.channels, "input_bytes": in_bytes,
         "frames": len(frames), "frames_per_stream": per_stream,
         "call_ms_median": call * 1e3, "call_ms_all": [t * 1e3 for t in times],
         "call_gsps": a.streams * a.samples / call / 1e9,
         "entry_ms_median": entry * 1e3, "entry_gsps": a.streams * a.samples / entry / 1e9,
+        "pinned_entry_ms_median": pinned * 1e3 if pinned else None,
+        "pinned_entry_gsps": a.streams * a.samples / pinned / 1e9 if pinned else None,
         "edges_kernel_ms": kt["edges"], "walk_kernel_ms": kt["walk"],
         "edges_bytes_per_s": in_bytes / (kt["edges"] / 1e3) if kt["edges"] else None,
         "edges_share_of_3.35TBps": in_bytes / (kt["edges"] / 1e3) / HBM_BYTES_PER_S if kt["edges"] else None,
