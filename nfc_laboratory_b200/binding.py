@@ -443,8 +443,10 @@ class NfcDecoder:
 
     def nextFrames(self, samples, sample_rate=None, sigtype=SIG_MAG_F32, cap=4096):
         """NfcDecoder::nextFrames(SignalBuffer): streaming decode of one capture.  samples=None (an invalid buffer in the
-        reference, NfcDecoder.cpp:449-463) flushes."""
+        reference, NfcDecoder.cpp:449-463) flushes.  Every frame the buffer completes is returned, however many: `cap` is
+        only the size of each copy out of the library."""
         rate = int(sample_rate or self._rate or 0)
+        cap = max(1, int(cap))
         buf = self._buffer(cap)
         n = C.c_uint64(0)
         if samples is None:
@@ -454,9 +456,16 @@ class NfcDecoder:
             a = np.ascontiguousarray(samples, dtype=dtype)
             count = a.size // comps
             rc = self._lib.nfcb200_stream_push(self._h, a.ctypes.data, sigtype, count, rate, buf, cap, C.byref(n))
-        _check(self._lib, rc)
+        if rc != -4:
+            _check(self._lib, rc)
         self._rate = rate
-        return self._convert(buf, n.value)
+        # more frames than cap: the push delivered cap of them, the rest wait in nfcb200_stream_pending
+        frames = self._convert(buf, n.value)
+        left = C.c_uint64(1 if rc == -4 else 0)
+        while left.value:
+            _check(self._lib, self._lib.nfcb200_stream_pending(self._h, buf, cap, C.byref(n), C.byref(left)))
+            frames += self._convert(buf, n.value)
+        return frames
 
     def stats(self):
         s = CStats()

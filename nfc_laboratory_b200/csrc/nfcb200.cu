@@ -1466,6 +1466,9 @@ int nfcb200_stream_push(nfcb200_handle *h, const void *samples, int sigtype, uin
       out[0].frame_type = FT_CarrierOff;
       out[0].frame_phase = PH_Carrier;
       out[0].sample_start = out[0].sample_end = 0xFFFFFFFFull;
+      // the reference divides that clock by its sample rate, still 0: the times are +inf like its frame's
+      out[0].time_start = out[0].time_end = (double) out[0].sample_start / (double) out[0].sample_rate;
+      out[0].date_time = (double) h->cfg.stream_time + out[0].time_start;
       if (n_out)
          *n_out = 1;
       return 0;

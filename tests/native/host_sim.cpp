@@ -91,11 +91,33 @@ int hostsim_carry_size(void)
    return (int) sizeof(Carry);
 }
 
+// decoder settings every later run takes (setup_params in nfcb200.cu): the power level and per tech the correlation and
+// modulation thresholds; hostsim_set_settings(NULL, ...) goes back to the reference defaults
+static bool g_settings = false;
+static float g_power;
+static TechThresholds g_thr[4];
+
+void hostsim_set_settings(const float *corr, const float *modMin, const float *modMax, float power)
+{
+   g_settings = corr != nullptr;
+   if (!g_settings)
+      return;
+   g_power = power;
+   for (int t = 0; t < 4; t++)
+      g_thr[t] = TechThresholds {corr[t], modMin[t], modMax[t]};
+}
+
 int hostsim_params(uint32_t sampleRate, uint32_t enabled, Params *P)
 {
    std::memset(P, 0, sizeof(*P));
    params_defaults(P);
    P->enabled = enabled;
+   if (g_settings)
+   {
+      P->power = g_power;
+      for (int t = 0; t < 4; t++)
+         P->thr[t] = g_thr[t];
+   }
    params_init(P, sampleRate);
    return P->valid;
 }
