@@ -219,6 +219,9 @@ struct nfcb200_handle
    struct NfcStream
    {
       nfcb200::DevBuf state, scratch, sbuf, samples, flags, bsum, pool, ext, counters;
+      nfcb200::DevBuf saved;                // state, scratch and sbuf as the current push found them
+      nfcb200::u32 poolCap = 1u << 14;      // frame pool: records, 128-byte extension chunks (grown to what a push needed)
+      nfcb200::u32 extCap = 1u << 12;
       std::vector<unsigned char> hostTail;  // samples retained on the host side of the stream buffer
       nfcb200::u32 base = 0;                // absolute index of the first retained sample
       nfcb200::u32 count = 0;               // retained samples

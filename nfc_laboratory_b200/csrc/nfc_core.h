@@ -939,6 +939,8 @@ struct Machine
    {
       if (size < 2)
          return true;
+      if (size > 512)
+         return false; // past the 512-byte buffer (the reference's CRC reads beyond its buffer[512]): a CRC error
       unsigned short crc = crc_ccitt16(sb, 0, size - 2, 0x6363, true);
       unsigned short res = (unsigned short) ((sb[size - 2] & 0xff) | ((sb[size - 1] & 0xff) << 8));
       return res == crc;
@@ -2137,6 +2139,8 @@ struct Machine
    {
       if (size < 3)
          return false;
+      if (size > 512)
+         return false; // past the 512-byte buffer (the reference's CRC reads beyond its buffer[512]): a CRC error
       unsigned short crc = (unsigned short) ~crc_ccitt16(sb, 0, size - 2, 0xFFFF, true);
       unsigned short res = (unsigned short) ((sb[size - 2] & 0xff) | ((sb[size - 1] & 0xff) << 8));
       return res == crc;
@@ -3250,6 +3254,8 @@ struct Machine
    {
       if (size < 3)
          return false;
+      if (size > 512)
+         return false; // past the 512-byte buffer (the reference's CRC reads beyond its buffer[512]): a CRC error
       unsigned short crc = (unsigned short) ~crc_ccitt16(sb, 0, size - 2, 0xFFFF, true);
       unsigned short res = (unsigned short) ((sb[size - 2] & 0xff) | ((sb[size - 1] & 0xff) << 8));
       return res == crc;

@@ -866,14 +866,20 @@ static int stream_decode(nfcb200_handle *h, bool flush, StreamState &hs)
       CUDA_TRY(cudaGetLastError());
    }
 
-   // frame pool for this push
+   // the lane's state as the push found it: a push whose frames overflow the pool is decoded again from here, in a pool
+   // grown to the need the counters report (they count past the caps; the decode is deterministic, so the second run
+   // gives the same frames)
+   const size_t stateBytes = sizeof(StreamState), scratchBytes = NFCB200_SCRATCH_FLOATS * sizeof(float);
+   if (int rc = S.saved.reserve(stateBytes + scratchBytes + 512))
+      return rc;
+   unsigned char *saved = S.saved.as<unsigned char>();
+   CUDA_TRY(cudaMemcpyAsync(saved, S.state.ptr, stateBytes, cudaMemcpyDeviceToDevice, st));
+   CUDA_TRY(cudaMemcpyAsync(saved + stateBytes, S.scratch.ptr, scratchBytes, cudaMemcpyDeviceToDevice, st));
+   CUDA_TRY(cudaMemcpyAsync(saved + stateBytes + scratchBytes, S.sbuf.ptr, 512, cudaMemcpyDeviceToDevice, st));
+
    Counters *dC = S.counters.as<Counters>();
    StreamConfig cfg;
    memset(&cfg, 0, sizeof(cfg));
-   if (int rc = frame_pool(S.pool, S.ext, 1u << 14, 1u << 12, dC, cfg.pool))
-      return rc;
-   CUDA_TRY(cudaMemsetAsync(dC, 0, sizeof(Counters), st));
-
    cfg.samples = S.samples.ptr;
    cfg.base = S.base;
    cfg.count = S.count;
@@ -887,16 +893,28 @@ static int stream_decode(nfcb200_handle *h, bool flush, StreamState &hs)
    cfg.scratch = S.scratch.as<float>();
    cfg.sbuf = S.sbuf.as<uint8_t>();
 
-   stream_kernel<<<1, 32, 0, st>>>(cfg, h->P);
-   CUDA_TRY(cudaGetLastError());
-
    Counters hc;
-   CUDA_TRY(cudaMemcpyAsync(&hc, dC, sizeof(Counters), cudaMemcpyDeviceToHost, st));
-   CUDA_TRY(cudaMemcpyAsync(&hs, S.state.ptr, sizeof(StreamState), cudaMemcpyDeviceToHost, st));
-   CUDA_TRY(cudaStreamSynchronize(st));
+   for (;;)
+   {
+      if (int rc = frame_pool(S.pool, S.ext, S.poolCap, S.extCap, dC, cfg.pool))
+         return rc;
+      CUDA_TRY(cudaMemsetAsync(dC, 0, sizeof(Counters), st));
 
-   if (hc.poolCount > cfg.pool.cap || hc.extCount > cfg.pool.extCap)
-      return fail(NFCB200_ERR_CAPACITY, "stream frame pool exhausted");
+      stream_kernel<<<1, 32, 0, st>>>(cfg, h->P);
+      CUDA_TRY(cudaGetLastError());
+
+      CUDA_TRY(cudaMemcpyAsync(&hc, dC, sizeof(Counters), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaMemcpyAsync(&hs, S.state.ptr, sizeof(StreamState), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+
+      if (hc.poolCount <= S.poolCap && hc.extCount <= S.extCap)
+         break;
+      S.poolCap = std::max(S.poolCap, hc.poolCount);
+      S.extCap = std::max(S.extCap, hc.extCount);
+      CUDA_TRY(cudaMemcpyAsync(S.state.ptr, saved, stateBytes, cudaMemcpyDeviceToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(S.scratch.ptr, saved + stateBytes, scratchBytes, cudaMemcpyDeviceToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(S.sbuf.ptr, saved + stateBytes + scratchBytes, 512, cudaMemcpyDeviceToDevice, st));
+   }
 
    std::vector<FrameRec> recs(hc.poolCount);
    std::vector<unsigned char> ext((size_t) hc.extCount * 128);
