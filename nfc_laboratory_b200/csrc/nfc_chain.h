@@ -204,6 +204,35 @@ struct LaneSucc
    }
 };
 
+// restart a lane at `target` from its own canonical carry (lane_iterate's skip-ahead), out of line: it runs a few times
+// per lane and takes no part in the register allocation of the step loop
+static NFC_HDN void lane_restart(Lane &L, const Params &P, u32 target, u32 kw)
+{
+   Carry carry = L.c;
+   carry.edgeTime = L.fe.edgeTime;
+   carry_canon(carry);
+   // what the run has recorded so far about its use of the INCOMING carry (chain_walk reads it) survives the restart:
+   // the run goes on from its own exact carry, it does not start a new dependency history
+   const u32 locked = L.lockedMask, lcWritten = L.lcWritten, lcLive = L.lcLive, fZeroed = L.fZeroed, fThrWritten = L.fThrWritten,
+             fThrRead = L.fThrRead, fInc00 = L.fInc0[0], fInc01 = L.fInc0[1];
+   const float fThrSync0 = L.fThrSync[0], fThrSync1 = L.fThrSync[1];
+   const u32 edgeWritten = L.edgeWritten, edgeLive = L.edgeLive;
+   lane_begin(L, P, carry, target, NFCB200_HALO);
+   L.lockedMask = locked;
+   L.lcWritten = lcWritten;
+   L.lcLive = lcLive;
+   L.fZeroed = fZeroed;
+   L.fThrWritten = fThrWritten;
+   L.fThrRead = fThrRead;
+   L.fInc0[0] = fInc00;
+   L.fInc0[1] = fInc01;
+   L.fThrSync[0] = fThrSync0;
+   L.fThrSync[1] = fThrSync1;
+   L.edgeWritten = edgeWritten;
+   L.edgeLive = edgeLive;
+   L.fe.kbase = kw;
+}
+
 /*
  * Drive one lane from R.first until it retires past R.end (or the stream ends).  Inside its own region the lane skips
  * idle stretches: when it is dormant outside every active block it jumps to HALO samples before the next active block
@@ -242,31 +271,9 @@ NFC_HD bool lane_iterate(MACH &M, Lane &L, const Params &P, u32 &pos, u32 &end, 
 
       if (begin > pos + NFCB200_HALO)
       {
-         Carry carry = L.c;
-         carry.edgeTime = L.fe.edgeTime;
-         carry_canon(carry);
-         // what the run has recorded so far about its use of the INCOMING carry (chain_walk reads it) survives the restart:
-         // the run goes on from its own exact carry, it does not start a new dependency history
-         const u32 locked = L.lockedMask, lcWritten = L.lcWritten, lcLive = L.lcLive, fZeroed = L.fZeroed, fThrWritten = L.fThrWritten,
-                   fThrRead = L.fThrRead, fInc00 = L.fInc0[0], fInc01 = L.fInc0[1];
-         const float fThrSync0 = L.fThrSync[0], fThrSync1 = L.fThrSync[1];
-         const u32 edgeWritten = L.edgeWritten, edgeLive = L.edgeLive;
-         u32 target = begin - NFCB200_HALO;
+         const u32 target = begin - NFCB200_HALO;
          zero();
-         lane_begin(L, P, carry, target, NFCB200_HALO);
-         L.lockedMask = locked;
-         L.lcWritten = lcWritten;
-         L.lcLive = lcLive;
-         L.fZeroed = fZeroed;
-         L.fThrWritten = fThrWritten;
-         L.fThrRead = fThrRead;
-         L.fInc0[0] = fInc00;
-         L.fInc0[1] = fInc01;
-         L.fThrSync[0] = fThrSync0;
-         L.fThrSync[1] = fThrSync1;
-         L.edgeWritten = edgeWritten;
-         L.edgeLive = edgeLive;
-         L.fe.kbase = kw;
+         lane_restart(L, P, target, kw);
          M.reload_front();
          pos = target;
       }

@@ -4187,7 +4187,9 @@ NFC_HD void group_copy(Carry &dst, Carry &src, int g)
 // start a lane at absolute sample index `first` (the first sample it will be fed).  first == 0 is the exact reference
 // start; otherwise this is the cold start of DESIGN.md: front end and rings restart from zero, carrier detection is
 // held off for `warm` local steps while the averages converge, detectors for NFCB200_RING steps as in the reference.
-NFC_HD void lane_begin(Lane &L, const Params &P, const Carry &carry, u32 first, u32 warm)
+// Out of line: it clears the whole Lane, and inlined into the thread lanes' kernel it set the register peak that made
+// the step loop spill (DESIGN.md §5).
+static NFC_HDN void lane_begin(Lane &L, const Params &P, const Carry &carry, u32 first, u32 warm)
 {
    u8 *raw = (u8 *) &L;
    for (u32 i = 0; i < sizeof(Lane); i++)
