@@ -288,6 +288,53 @@ int nfcb200_iso7816_stream_pending(nfcb200_handle *h, nfcb200_frame *out, uint64
 /* forget the ISO stream: the next push decodes as on a fresh handle (the sample before it is 0) */
 int nfcb200_iso7816_stream_reset(nfcb200_handle *h);
 
+/* one point of the reference's adaptive signal (lab::SignalResamplingTask): the sample at stream position `sample` kept
+ * with its value.  `stream` is the batch index, `channel` 0 for radio and the logic channel for logic. */
+typedef struct nfcb200_signal_point
+{
+   uint32_t stream;
+   uint32_t channel;
+   uint64_t sample;
+   float value;
+   uint32_t reserved;
+} nfcb200_signal_point;
+
+/*
+ * The adaptive signal of radio captures: lab::SignalResamplingTask::processRadioSignal (lab-tasks
+ * SignalResamplingTask.cpp:168-229), the waveform of the reference GUI's signal view (QtControl.cpp:238, 296) and the
+ * radio signal TraceStorageTask stores in a .trz (TraceStorageTask.cpp:881-1003).  n_streams captures of n_samples each,
+ * laid out [n_streams][n_samples] in `sigtype` format (any radio format; IQ enters as its magnitude sqrtf(I*I + Q*Q),
+ * int16 as s / 32768.f), are cut into buffers of buffer_len samples (the last one of a stream shorter), each resampled on
+ * its own as the reference resamples each buffer it is handed: replayed files come in buffers of 65 536 samples
+ * (SignalStorageTask.cpp:323-437).  A live capture is one call per buffer with n_streams = 1, buffer_len = n_samples and
+ * `offset` the position of its first sample: the reference keeps no state across buffers.
+ *   points: ordered by (stream, emission order of the reference); sample = offset + buffer start + (unsigned) float(i),
+ *           the index i stored as float as the reference stores it.  More points than cap: NFCB200_ERR_CAPACITY after
+ *           filling cap, *n_out the total.  `out` is host memory.
+ *   where the reference is undefined: a buffer shorter than 25 samples reads past its end in the reference's initial sum,
+ *           here those samples are 0; a buffer yields at most buffer_len + 1 points, which is more than the reference's
+ *           output buffer holds (:170, it writes past it) for a buffer under 255 samples whose samples all deviate,
+ *           here every point is returned.
+ * Invalid sigtype, a null handle, an empty batch, buffer_len 0 or a sample rate of 0: NFCB200_ERR_INVALID.  buffer_len
+ * over 2^24 (indices would not be exact as float) or a stream reaching position 2^32 (the .trz's 32-bit offsets):
+ * NFCB200_ERR_UNSUPPORTED.  The call changes no decode state of the handle.
+ */
+int nfcb200_adaptive_radio(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t n_streams, uint64_t n_samples,
+                           uint32_t sample_rate, uint64_t buffer_len, uint64_t offset, nfcb200_signal_point *out, uint64_t cap, uint64_t *n_out);
+
+/*
+ * The adaptive signal of logic captures: lab::SignalResamplingTask::processLogicSignal (SignalResamplingTask.cpp:231-274),
+ * stored by TraceStorageTask as logic-<channel>.apcm (TraceStorageTask.cpp:643-758).  Captures of `channels` channels (4-8)
+ * laid out [n_streams][n_samples][channels] in NFCB200_SIG_LOGIC_F32, _S16 (s / 32768.f) or _U8 (b / 255.f), cut into
+ * buffers as nfcb200_adaptive_radio cuts them.  Every channel but 1 (CLK) gets its points: the first sample of each buffer,
+ * each sample that differs from the one before it, and one sample 255 after each point kept.  Points are ordered by
+ * (stream, channel, emission order), `channel` the channel number.  Device samples must be aligned to one element.
+ * Every other convention is nfcb200_adaptive_radio's; channels outside 4-8 returns NFCB200_ERR_INVALID.
+ */
+int nfcb200_adaptive_logic(nfcb200_handle *h, const void *samples, int samples_on_device, int sigtype, uint32_t channels, uint32_t n_streams,
+                           uint64_t n_samples, uint32_t sample_rate, uint64_t buffer_len, uint64_t offset, nfcb200_signal_point *out, uint64_t cap,
+                           uint64_t *n_out);
+
 const char *nfcb200_last_error(void);
 
 /* library / build identification, e.g. "nfcb200 0.1 sm_90a" */

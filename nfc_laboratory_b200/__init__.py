@@ -8,6 +8,7 @@ from .binding import (  # noqa: F401
     Frame,
     NfcB200Error,
     NfcDecoder,
+    SIGNAL_POINT_DTYPE,
     SIG_IQ_F32,
     SIG_IQ_S16,
     SIG_LOGIC_F32,
@@ -22,5 +23,5 @@ from .binding import (  # noqa: F401
 from .logic_wav import LogicWav, read_logic_wav, write_logic_wav  # noqa: F401
 
 __all__ = ["Frame", "NfcB200Error", "NfcDecoder", "SIG_IQ_F32", "SIG_MAG_F32", "SIG_MAG_S16", "SIG_IQ_S16", "SIG_LOGIC_F32", "SIG_LOGIC_S16",
-           "SIG_LOGIC_U8", "LogicWav", "read_logic_wav", "write_logic_wav", "library_path",
+           "SIG_LOGIC_U8", "SIGNAL_POINT_DTYPE", "LogicWav", "read_logic_wav", "write_logic_wav", "library_path",
            "load_library", "spectrum_shape"]

@@ -82,7 +82,12 @@ EXPORTS = [
     "nfcb200_stream_push", "nfcb200_stream_reset", "nfcb200_get_stats", "nfcb200_get_block_flags", "nfcb200_pack_frames",
     "nfcb200_last_error", "nfcb200_version", "nfcb200_device_frames", "nfcb200_emit_records", "nfcb200_stream_pending", "nfcb200_debug_trace", "nfcb200_carry_size", "nfcb200_set_carry",
     "nfcb200_carry_before", "nfcb200_default_carry", "nfcb200_spectrum", "nfcb200_spectrum_shape",
+    "nfcb200_adaptive_radio", "nfcb200_adaptive_logic",
 ]
+
+# nfcb200_signal_point: one point of the adaptive signal (NfcDecoder.adaptive_radio / adaptive_logic)
+SIGNAL_POINT_DTYPE = np.dtype([("stream", "<u4"), ("channel", "<u4"), ("sample", "<u8"), ("value", "<f4"), ("reserved", "<u4")])
+ADAPTIVE_BUFFER = 65536  # samples per buffer of a replayed file (SignalStorageTask.cpp:323-437)
 
 SPECTRUM_BINS = 1024
 
@@ -137,6 +142,10 @@ def load_library():
                                                    C.c_uint64, C.POINTER(C.c_uint64)]
     lib.nfcb200_iso7816_stream_pending.argtypes = [C.c_void_p, C.POINTER(CFrame), C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     lib.nfcb200_iso7816_stream_reset.argtypes = [C.c_void_p]
+    lib.nfcb200_adaptive_radio.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint64,
+                                           C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.nfcb200_adaptive_logic.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32,
+                                           C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.nfcb200_spectrum_shape.argtypes = [C.c_uint64, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
     _lib = lib
     return lib
@@ -388,6 +397,45 @@ class NfcDecoder:
         _check(self._lib, self._lib.nfcb200_spectrum(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams, n_samples, int(sample_rate),
                                                      int(hop), C.c_void_p(out_ptr), 1 if out_on_device else 0, int(cap), C.byref(nf)))
         return int(nf.value)
+
+    def adaptive_radio(self, samples, sigtype, sample_rate, buffer=ADAPTIVE_BUFFER, offset=0):
+        """the reference's adaptive signal of radio captures (lab::SignalResamplingTask, the GUI's signal view): numpy
+        [n_streams, n_samples] magnitude or [n_streams, n_samples, 2] IQ (or one stream without the first axis), or a torch
+        tensor of that shape, cut into buffers of `buffer` samples, the stream's first sample at position `offset`.
+        Returns a SIGNAL_POINT_DTYPE array ordered by (stream, emission order) (include/nfcb200.h nfcb200_adaptive_radio)."""
+        a, ptr, on_device = self._batch(samples, sigtype)
+        n_streams, n_samples = int(a.shape[0]), int(a.shape[1])
+        return self._points(lambda out, cap, n: self._lib.nfcb200_adaptive_radio(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, n_streams,
+                                                                                 n_samples, int(sample_rate), int(buffer), int(offset), out, cap, n),
+                            n_streams * n_samples)
+
+    def adaptive_logic(self, samples, sigtype, sample_rate, channels=None, buffer=ADAPTIVE_BUFFER, offset=0):
+        """the adaptive signal of logic captures [n_streams, n_samples, C] (or one stream [n_samples, C]), C = 4-8 channels
+        in a logic format as iso7816_decode takes them; channels=None takes C from the shape.  Every channel but 1 (CLK) has
+        points.  Returns a SIGNAL_POINT_DTYPE array ordered by (stream, channel, emission order)."""
+        _logic_dtype(samples, sigtype)
+        a, ptr, on_device = self._batch(samples, sigtype)
+        if len(a.shape) != 3 or (channels is not None and int(channels) != a.shape[2]):
+            raise NfcB200Error(-2, "logic samples must be [n_streams, n_samples, channels], got %s" % (tuple(a.shape),))
+        n_streams, n_samples, ch = int(a.shape[0]), int(a.shape[1]), int(a.shape[2])
+        return self._points(lambda out, cap, n: self._lib.nfcb200_adaptive_logic(self._h, C.c_void_p(ptr), 1 if on_device else 0, sigtype, ch,
+                                                                                 n_streams, n_samples, int(sample_rate), int(buffer), int(offset),
+                                                                                 out, cap, n),
+                            n_streams * n_samples * max(1, ch - 1))
+
+    def _points(self, call, n_in):
+        """call(out, cap, byref(n)) of an adaptive entry point, again with room for every point when the first guess (a
+        quiet signal keeps about one sample in 255) was too small"""
+        cap = n_in // 128 + 1024
+        while True:
+            out = np.empty(cap, dtype=SIGNAL_POINT_DTYPE)
+            n = C.c_uint64(0)
+            rc = call(C.c_void_p(out.ctypes.data), cap, C.byref(n))
+            if rc == -4 and n.value > cap:
+                cap = int(n.value)
+                continue
+            _check(self._lib, rc)
+            return out[: n.value]
 
     def iso7816_decode(self, samples, sigtype, sample_rate, cap=1 << 16, raw=False):
         """ISO 7816 contact smart-card frames (lab::IsoDecoder) of logic captures of C = 4-8 channels, IO, CLK, RST, VCC first:

@@ -238,6 +238,13 @@ struct nfcb200_handle
       bool tablesReady = false;
    } spec;
 
+   // nfcb200_adaptive_radio / nfcb200_adaptive_logic: buffers of their own too
+   struct Adaptive
+   {
+      nfcb200::DevBuf in, count, first, out; // staged host input, points per list, their places, points of one window
+      nfcb200::HostBuf hCount;               // points per list on the host
+   } adapt;
+
    // the ISO 7816 dense pass's per-tile event slots and counts (iso_decode.cuh)
    struct IsoEvents
    {
